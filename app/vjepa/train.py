@@ -1,7 +1,7 @@
 """V-JEPA pre-training loop: `app.vjepa.train.main(args, resume_preempt=False)`.
 
 Same config schema, schedules, CSV columns, log lines and checkpoint format as the reference
-(app/vjepa/train.py), with the math of every step running on the sm_100a kernels of jepa_b200:
+(app/vjepa/train.py), with the math of every step running on the sm_90a kernels of jepa_b200:
   target forward + LN + gather  -> jepa_b200.step.forward_target      (train.py:419-429)
   context encoder + predictor   -> fused multi-mask passes            (train.py:431-438)
   L1 latent loss / variance reg -> jepa_b200.step.jepa_loss/reg_loss  (train.py:440-459)
@@ -61,7 +61,7 @@ def main(args, resume_preempt=False):
     if which_dtype.lower() == 'bfloat16':
         dtype, mixed_precision = torch.bfloat16, True
     elif which_dtype.lower() == 'float16':
-        raise NotImplementedError("dtype float16: the tcgen05 kernels compute bf16 x bf16 -> fp32 only")
+        raise NotImplementedError("dtype float16: the wgmma kernels compute bf16 x bf16 -> fp32 only")
     else:
         raise NotImplementedError("dtype float32: there is no fp32 tensor-core path; use dtype: bfloat16 "
                                   "(the configuration of every shipped pre-training config)")
@@ -139,7 +139,7 @@ def main(args, resume_preempt=False):
     logger.info(f'Initialized (rank/world-size) {rank}/{world_size}')
 
     if not torch.cuda.is_available():
-        raise RuntimeError("app.vjepa.train: a CUDA (sm_100a) device is required - the training step has no CPU path")
+        raise RuntimeError("app.vjepa.train: a CUDA (sm_90a) device is required - the training step has no CPU path")
     device = torch.device('cuda:0')
     torch.cuda.set_device(device)
 

@@ -2,6 +2,7 @@
 """Headline benchmark: V-JEPA pre-training step, clips/sec, ViT-L/16 16x224x224 synthetic, B=32 per GPU.
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--config vitl16|vith16|vith16_384|tiny]
+                    [--dump-outputs DIR]
     torchrun --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 --master-port P bench.py --gpus N ...
 
 A "step" is everything inside the reference's train_step() (app/vjepa/train.py:414-498) minus the three
@@ -9,9 +10,11 @@ logging helpers (grad_logger x2, adamw_logger): LR/WD schedule, target forward +
 encoder + predictor forward/backward, L1 loss, GradScaler, AdamW, zero_grad, EMA; N>1 adds the DDP gradient
 all-reduce.  `value` times K such steps with inputs resident in HBM (CUDA events, max over ranks); `e2e`
 repeats them through the public module API with HOST inputs: pinned clips + masks copied to the device and
-the loss read back every step.  `--impl reference` times the UNMODIFIED reference's CPU path (baseline/_ref, its own
-app.vjepa.train.main, fp32) on the host cores; if baseline/_ref is absent it falls back to the CPU oracle port.
-Prints ONE JSON line on rank 0.
+the loss read back every step.  `--impl reference` times the UNMODIFIED reference's CPU path (oracle/_ref, its own
+app.vjepa.train.main, fp32) on the host cores; if oracle/_ref is absent it falls back to the CPU oracle port.
+Prints ONE JSON line on rank 0.  `--dump-outputs DIR` writes what the last timed step produced (loss, and a fixed
+seeded sample of the updated encoder / predictor / target weights) as DIR/<name>.npy, so two builds can be compared
+output for output on identical inputs.
 """
 import argparse
 import json
@@ -81,11 +84,12 @@ def measured_peaks():
             d = json.load(f)
         return dict(bf16_burst=d.get("bf16_tflops"), bf16_sustained=d.get("bf16_tflops_sustained"),
                     hbm_gbs=d.get("hbm_gbs"), source="measured")
-    return dict(bf16_burst=1590.0, bf16_sustained=1400.0, hbm_gbs=6650.0, source="fallback")
+    # NVIDIA's H100 SXM data sheet (dense BF16, HBM3) - limits, not measurements
+    return dict(bf16_burst=989.0, bf16_sustained=989.0, hbm_gbs=3350.0, source="H100 SXM data sheet")
 
 
 class ClockSampler:
-    """nvidia-smi sampling DURING the timed region (B200_PROFILING.md clocks line)."""
+    """nvidia-smi sampling DURING the timed region: SM clock and throttle reasons of the measured steps."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
          "clocks_event_reasons.sw_power_cap")
@@ -237,19 +241,27 @@ def ddp_gradient_check(st, clips, masks_enc, masks_pred):
                 n_grad_elements=int(g_mean.numel()))
 
 
-def ncu_gemm_traffic(cfg_name):
-    """DRAM bytes moved by the GEMM family in one step, from the committed ncu launch list of `bench.py --profile`
-    (profiles/, vitl16 only); None when no capture exists for this config."""
-    prof = os.path.join(os.path.dirname(os.path.abspath(__file__)), "profiles")
-    path = next((p for p in (os.path.join(prof, "r02_step_launches_summary.txt"),
-                             os.path.join(prof, "r01_step_launches_final_summary.txt")) if os.path.exists(p)), "")
-    if cfg_name != "vitl16" or not path:
-        return None
-    with open(path) as f:
-        for line in f:
-            if line.startswith("# gemm family:"):
-                return int(float(line.split("DRAM traffic")[1].split("GB")[0]) * 1e9)
-    return None
+DUMP_SAMPLE = 1 << 20   # weights sampled per module by --dump-outputs (4 MB of fp32 + 8 MB of indices each)
+
+
+def dump_outputs(out_dir, st, loss):
+    """What a caller of train_step receives after the last timed step: the loss and the updated weights (encoder,
+    predictor, EMA target), the weights as a fixed seeded sample of their flattened parameter order."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    np.save(os.path.join(out_dir, "loss.npy"), np.array([float(loss)], dtype=np.float64))
+    for name in ("encoder", "predictor", "target"):
+        params = [p.detach().reshape(-1) for p in st[name].parameters()]
+        total = sum(p.numel() for p in params)
+        idx = torch.randint(0, total, (min(DUMP_SAMPLE, total),), generator=torch.Generator().manual_seed(0)).sort().values
+        parts, off = [], 0
+        for p in params:
+            lo, hi = torch.searchsorted(idx, torch.tensor([off, off + p.numel()]))
+            if hi > lo:
+                parts.append(p[(idx[lo:hi] - off).to(p.device)].float().cpu())
+            off += p.numel()
+        np.save(os.path.join(out_dir, f"{name}_weights_sample.npy"), torch.cat(parts).numpy())
+        np.save(os.path.join(out_dir, f"{name}_weights_sample_index.npy"), idx.numpy().astype(np.float64))
 
 
 def run_ours(args):
@@ -325,13 +337,15 @@ def run_ours(args):
     launches = lib.vj_launch_count() - launches0
     clocks = sampler.stop() if sampler else None
     last_loss = float(loss)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, st, loss)
     if world > 1:
         t = torch.tensor([ms_total], device=device)
         dist.all_reduce(t, op=dist.ReduceOp.MAX)
         ms_total = float(t)
     ms_step = ms_total / args.steps
     value = B * world / (ms_step * 1e-3)
-    if args.profile:   # run under ncu: only the bare steps, no auxiliary passes
+    if args.profile:   # run under a profiler: only the bare steps, no auxiliary passes
         if rank == 0:
             print(json.dumps({"profile_run": True, "ms_per_step": ms_step, "gpu_launches": int(launches)}), flush=True)
         return
@@ -437,7 +451,7 @@ def run_ours(args):
                                    f"multiblock3d masks Ke={Ke} Kp={Kp} (seed 0, first collator call), predictor 12x384, "
                                    "AdamW+GradScaler+EMA in step, logging helpers off",
                        "global_batch": B * world, "parallelism": f"dp{world}",
-                       "l2_policy": "inputs+weights+activations per step (>3 GB) exceed the 126 MB L2; no explicit flush",
+                       "l2_policy": "inputs+weights+activations per step (>3 GB) exceed the 50 MB L2; no explicit flush",
                        "flops_per_clip": f_clip, "loss_last": last_loss},
             "clocks": clocks,
             "e2e": {"value": round(e2e_value, 2), "unit": "clips/s", "h2d_bytes_per_step": h2d, "d2h_bytes_per_step": 4},
@@ -447,7 +461,7 @@ def run_ours(args):
                 "bound": "tensor", "scope": "whole train step (BASELINE metric: % tensor-pipe roofline of the step)",
                 "achieved": round(step_tf, 1), "peak": peak, "unit": "TFLOP/s", "frac": round(step_tf / peak, 4),
                 "peak_source": f"{peaks['source']} bf16_tflops_sustained (kernel timed inside a long step)",
-                "frac_of_burst": round(step_tf / peaks["bf16_burst"], 4), "frac_of_nominal_2250": round(step_tf / 2250.0, 4),
+                "frac_of_burst": round(step_tf / peaks["bf16_burst"], 4),
                 "algorithmic_tflop_per_step": round(f_clip * B / 1e12, 3),
                 "dominant_kernel": {
                     "kernel": "vj::gemm_kernel (all Linear / patch-embed GEMMs of a step)", "achieved": round(achieved, 1),
@@ -459,10 +473,7 @@ def run_ours(args):
                     "kernel": "vj::attn_fwd/bwd kernels", "fwd_ms_per_step": round(attn_fwd_ms, 3),
                     "bwd_ms_per_step": round(attn_bwd_ms, 3), "algorithmic_tflop_per_step": round(fa_clip * B / 1e12, 3),
                     "achieved": round(fa_clip * B / ((attn_fwd_ms + attn_bwd_ms) * 1e-3) / 1e12, 1),
-                    "frac": round(fa_clip * B / ((attn_fwd_ms + attn_bwd_ms) * 1e-3) / 1e12 / peak, 4)},
-                "traffic": ncu_gemm_traffic(args.config),
-                "traffic_unit": "DRAM bytes per step over the GEMM family's launches (dram__bytes_read.sum + "
-                                "dram__bytes_write.sum, ncu launch list in profiles/)"},
+                    "frac": round(fa_clip * B / ((attn_fwd_ms + attn_bwd_ms) * 1e-3) / 1e12 / peak, 4)}},
         }
         if ddp_check is not None:
             line["ddp_check"] = ddp_check
@@ -542,11 +553,11 @@ def usable_cores():
 
 
 def reference_cpu_run(cfg_name, B, steps, warmup, cores, timeout=1500):
-    """The UNMODIFIED reference (baseline/_ref, tools/install_reference.sh) through its own app.vjepa.train.main on the
+    """The UNMODIFIED reference (oracle/_ref, oracle/make_ref.sh) through its own app.vjepa.train.main on the
     host cores: fp32 (CPU autocast / GradScaler disable themselves), AdamW + EMA + its loggers in the step, synthetic clips,
     its own collator - SURVEY 8d's CPU baseline.  Runs in a subprocess (tools/ref_gpu.py --backend gloo) because the
-    repo's drop-in src/ and app/ packages carry the reference's module names.  None if baseline/_ref is absent."""
-    if not os.path.isdir(os.path.join(ROOT, "baseline", "_ref", "app")):
+    repo's drop-in src/ and app/ packages carry the reference's module names.  None if oracle/_ref is absent."""
+    if not os.path.isdir(os.path.join(ROOT, "oracle", "_ref", "app")):
         return None
     cmd = [sys.executable, os.path.join(ROOT, "tools", "ref_gpu.py"), "bench", "--config", cfg_name, "--backend", "gloo",
            "--batch", str(B), "--steps", str(steps), "--warmup", str(warmup), "--loggers", "on", "--threads", str(cores)]
@@ -569,7 +580,7 @@ def cpu_baseline(cfg_name, budget_s=25.0):
     ref = reference_cpu_run(cfg_name, B=2, steps=2, warmup=1, cores=cores)   # ~3 steps of 5-10 s at ViT-L
     if ref is not None:
         return {"value": ref["clips_per_s"], "unit": "clips/s", "cores": cores, "kind": "reference", "adamw": True,
-                "sample": f"unmodified reference app.vjepa.train.main (baseline/_ref) on the host: 2 timed fp32 steps (+1 warm-up) "
+                "sample": f"unmodified reference app.vjepa.train.main (oracle/_ref) on the host: 2 timed fp32 steps (+1 warm-up) "
                           f"at batch 2 of {cfg_name}, median {ref['gpu_ms_per_step_median'] / 1e3:.2f} s/step by its own "
                           f"wall-time column, AdamW/EMA/loggers in the step, {cores} torch threads"}
     torch.set_num_threads(cores)
@@ -605,7 +616,7 @@ def run_reference(args):
         value = ref["clips_per_s"]
         ms_step = ref["gpu_ms_per_step_median"]
         loss = ref["losses"][-1]
-        sample = (f"each step = one fp32 train step of the UNMODIFIED reference (baseline/_ref, app.vjepa.train.main: target fwd, "
+        sample = (f"each step = one fp32 train step of the UNMODIFIED reference (oracle/_ref, app.vjepa.train.main: target fwd, "
                   f"context+predictor fwd/bwd, AdamW, EMA, its loggers) on {B} clips of {args.config} ({model_name}, "
                   f"{frames}x{crop}x{crop}, its own MaskCollator at batch {B}); median of {args.steps} by its wall-time column; "
                   f"{cores} host threads")
@@ -622,7 +633,7 @@ def run_reference(args):
         dt = time.perf_counter() - t0
         value = B * args.steps / dt
         ms_step = dt / args.steps * 1e3
-        sample = (f"baseline/_ref absent -> CPU oracle port: each step = one fp32 train step (AdamW omitted) on {B} clip of "
+        sample = (f"oracle/_ref absent -> CPU oracle port: each step = one fp32 train step (AdamW omitted) on {B} clip of "
                   f"{args.config} ({model_name}, {frames}x{crop}x{crop}, masks Ke={Ke} Kp={Kp}); {cores} host threads")
     line = {
         "impl": "reference",
@@ -652,7 +663,9 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--dynamic-masks", action="store_true", help="new collator call every step (SURVEY 8d second run)")
     ap.add_argument("--loggers", action="store_true", help="as-shipped step: grad_logger x2 + adamw_logger inside the step")
-    ap.add_argument("--profile", action="store_true", help="bare steps only (for ncu); never a bench value")
+    ap.add_argument("--profile", action="store_true", help="bare steps only (for a profiler); never a bench value")
+    ap.add_argument("--dump-outputs", default="", metavar="DIR",
+                    help="write the last timed step's loss and a seeded sample of the updated weights as DIR/<name>.npy")
     args = ap.parse_args()
     if args.impl == "reference":
         args.steps = args.steps if args.steps is not None else 3

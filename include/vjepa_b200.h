@@ -1,4 +1,4 @@
-/* vjepa_b200.h - C ABI of the B200-native V-JEPA pre-training hot path (libvjepa_b200.so).
+/* vjepa_b200.h - C ABI of the H100-native V-JEPA pre-training hot path (libvjepa_b200.so).
  *
  * The reference (facebookresearch/jepa) is pure Python: it has no FFI layer, its hot path is the
  * set of torch library calls listed in SURVEY.md section 2.3 (K1..K15).  Every entry point below
@@ -42,7 +42,7 @@ int vj_set_sm_limit(int n);
 /* CUtensorMap cache statistics: which = 0 -> hits, 1 -> misses (driver encode calls) since the library was loaded. */
 long long vj_tmap_cache_stats(int which);
 
-/* D[M,N] = epi(alpha * A[M,K] . B[N,K]^T), bf16 operands, fp32 accumulate (tcgen05 / TMEM).
+/* D[M,N] = epi(alpha * A[M,K] . B[N,K]^T), bf16 operands, fp32 accumulate (wgmma).
  * a_mn = 0: A stored [M,K] (K contiguous, ld = lda);  a_mn = 1: A stored [K,M] (M contiguous).
  * b_mn = 0: B stored [N,K];                            b_mn = 1: B stored [K,N].
  * Supported (a_mn,b_mn): (0,0) forward / nn.Linear, (0,1) dgrad, (1,1) wgrad.
@@ -61,7 +61,7 @@ int vj_gemm(const void* A, long long lda, int a_mn, const void* B, long long ldb
             int aux_period, void* aux_out, long long ldauxout, int split_k, int accumulate,
             void* stream);
 
-/* Dense var-len flash attention forward (tcgen05).  qkv bf16 [T, 3*H*HD] (q|k|v thirds, head-major),
+/* Dense var-len flash attention forward (wgmma).  qkv bf16 [T, 3*H*HD] (q|k|v thirds, head-major),
  * out bf16 [T, H*HD], lse2 fp32 [H, T] (log2 domain).  Sequences are the row ranges
  * [cu_seqlens[s], cu_seqlens[s+1]) (device int32 [nseq+1]); max_len = longest sequence.
  * HD in {32, 64, 128} (hd=24 heads are zero-padded to 32 by the weight layout).
@@ -70,8 +70,7 @@ int vj_attn_fwd(const void* qkv, void* out, float* lse2, const int* cu_seqlens, 
                 int H, int HD, int T, float scale, void* stream);
 
 /* Backward of the above: dqkv bf16 [T, 3*H*HD] from dout bf16 [T, H*HD]; delta_ws fp32 [H*T] scratch.
- * dq_acc_ws: optional fp32 [T, H*HD] scratch; when given and HD <= 32 the dQ computation is fused into the
- * dK/dV kernel (TMA reduce-add of per-key-tile partials) instead of a second recomputing kernel.
+ * dq_acc_ws: unused (may be NULL); kept so callers built against earlier versions of this header still link.
  * (autograd of modules.py:66-69). */
 int vj_attn_bwd(const void* qkv, const void* out, const void* dout, const float* lse2, float* delta_ws,
                 void* dqkv, float* dq_acc_ws, const int* cu_seqlens, int nseq, int max_len, int H, int HD, int T,
@@ -155,7 +154,7 @@ int vj_cross_attn_fwd(const void* q, const void* kv, void* out, int B, int nq, i
 int vj_cast_f32_bf16(const float* src, void* dst, long long n, void* stream);
 /* Tensors viewed as [outer, G, hd, inner] <-> [outer, G, hdp, inner]: zero-pad heads (unpad_add=0) or
  * accumulate the padded fp32 gradient back into the unpadded one (unpad_add=1).  Predictor heads are
- * hd = 384/16 = 24 (app/vjepa/utils.py:119) and run as 32-wide tcgen05 tiles. */
+ * hd = 384/16 = 24 (app/vjepa/utils.py:119) and run as 32-wide wgmma tiles. */
 int vj_head_pad(const void* src, int src_f32, void* dst, int dst_f32, long long outer, int G, int hd, int hdp,
                 long long inner, int unpad_add, void* stream);
 /* k = k*m + one_minus_m*q over a flat fp32 buffer, rounding op-for-op like

@@ -1,4 +1,4 @@
-"""jepa_b200: B200-native (sm_100a) V-JEPA pre-training hot path.
+"""jepa_b200: H100-native (sm_90a) V-JEPA pre-training hot path.
 
 csrc/ holds the hand-written CUDA kernels behind the C ABI of include/vjepa_b200.h; the Python
 modules mirror the reference's src/ and app/ API on top of it.  PyTorch provides device memory,

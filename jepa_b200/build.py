@@ -1,7 +1,7 @@
-"""Build the C-ABI shared library (libvjepa_b200.so) in-tree with nvcc for sm_100a.
+"""Build the C-ABI shared library (libvjepa_b200.so) in-tree with nvcc for sm_90a (H100).
 
-The built .so is git-ignored but travels to the GPU box with the gpurun snapshot.  No torch
-headers are involved: the library is a plain C ABI over raw device pointers (include/vjepa_b200.h).
+The built .so and objects are git-ignored build products.  No torch headers are involved: the
+library is a plain C ABI over raw device pointers (include/vjepa_b200.h).
 """
 import hashlib
 import os
@@ -15,7 +15,7 @@ LIB = os.path.join(HERE, "libvjepa_b200.so")
 OBJ_DIR = os.path.join(HERE, "build")
 
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-ARCH = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 FLAGS = ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC",
          "-I" + os.path.join(ROOT, "include"), "-I" + CSRC]
 

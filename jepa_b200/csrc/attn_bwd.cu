@@ -1,15 +1,14 @@
-// Flash-attention backward on tcgen05 / TMEM (sm_100a), dense var-len, deterministic (no atomics).
+// Flash-attention backward on wgmma (sm_90a), dense var-len, deterministic (no atomics).
 //
 // Backward of F.scaled_dot_product_attention (src/models/utils/modules.py:66-69):
 //   P = softmax(scale Q K^T), dV = P^T dO, dP = dO V^T, dS = P o (dP - rowsum(dO o O)),
 //   dQ = scale dS K, dK = scale dS^T Q.
 // Three kernels:
-//   attn_delta_kernel : delta[h,t] = sum_d dO[t,h,d] O[t,h,d]                      (HBM-bound)
-//   attn_bwd_dkv_kernel: one CTA per 128-key tile, loops over query tiles; computes S^T = K Q^T and
-//                        dP^T = V dO^T directly in the transposed orientation so P^T / dS^T are the
-//                        M-side (K-major) operands of dV += P^T dO and dK += dS^T Q, both accumulated
-//                        in TMEM across the whole loop.
-//   attn_bwd_dq_kernel : one CTA per 128-query tile, loops over key tiles; dQ += dS K in TMEM.
+//   attn_delta_kernel  : delta[h,t] = sum_d dO[t,h,d] O[t,h,d]                      (HBM-bound)
+//   attn_bwd_dkv_kernel: one CTA per 128-key tile (two warpgroups of 64 keys), loops over 64-query tiles; computes
+//                        S^T = K Q^T and dP^T = V dO^T directly in the transposed orientation so P^T / dS^T are register
+//                        A operands of dV += P^T dO and dK += dS^T Q, both accumulated in registers across the loop.
+//   attn_bwd_dq_kernel : one CTA per 128-query tile, loops over 64-key tiles; dQ += dS K in registers.
 // P is recomputed from the forward's log2-domain LSE.  Same qkv / O layouts as attn_fwd.cu; the
 // gradient dqkv has the qkv layout [T, 3*H*HD] so the qkv wgrad/dgrad GEMMs consume it directly.
 #include <stdlib.h>
@@ -18,6 +17,9 @@
 #include "vjepa_b200.h"
 
 namespace vj {
+
+constexpr int kBwdThreads = 256;
+constexpr int kBwdStream = 64;   // rows of the streamed (query or key) tiles
 
 struct AttnBwdParams {
   const int* cu_seqlens;
@@ -31,23 +33,14 @@ struct AttnBwdParams {
 template <int HD>
 struct BwdCfg {
   using A = AttnCfg<HD>;
-  // two resident [128 x HD] operand tiles (T0, T1), ST stages of the two streamed tiles, one [128 x 128] bf16
-  // P/dS tile, stats, barriers.  The streamed pair is double-buffered when it is small enough (HD <= 32) to keep
-  // two CTAs per SM: its TMA latency then hides behind the previous iteration instead of sitting on the chain.
-  static constexpr int ST = HD <= 32 ? 2 : 1;
-  static constexpr int T0 = 0, T1 = A::TILE_BYTES, T2 = 2 * A::TILE_BYTES, T3 = 3 * A::TILE_BYTES;
-  static constexpr int STAGE_BYTES = 2 * A::TILE_BYTES;
-  static constexpr int PS_OFF = (2 + 2 * ST) * A::TILE_BYTES;
-  static constexpr int STAT_OFF = PS_OFF + A::P_BYTES;        // [2][2][128] floats
-  static constexpr bool CAN_FUSE_DQ = HD <= 32;               // S^T + dV + dK + dQ partial fit 256 TMEM columns
-  static constexpr int DQS_OFF = STAT_OFF + 2 * 2 * 128 * 4;  // 4 warps x [32 rows x 32 fp32] dQ-partial staging
-  static constexpr int BAR_OFF = DQS_OFF + (CAN_FUSE_DQ ? 4 * 4096 : 0);
-  static constexpr int SMEM_BYTES = BAR_OFF + 128 + 1024;
-  static constexpr int DKV_TMEM = (128 + (CAN_FUSE_DQ ? 3 : 2) * HD) <= 256 ? 256 : 512;
-  static constexpr int DQ_TMEM = (128 + HD) <= 256 ? 256 : 512;
+  // two resident [128 x HD] tiles (T0, T1) and two stages of the two streamed [64 x HD] tiles
+  static constexpr int RES = A::template tile_bytes<128>();
+  static constexpr int STR = A::template tile_bytes<kBwdStream>();
+  static constexpr int T0 = 0, T1 = RES;
+  static constexpr int S_OFF = 2 * RES;                 // stage st: tile a at S_OFF + st * 2 * STR, tile b at + STR
+  static constexpr int BAR_OFF = S_OFF + 4 * STR;
+  static constexpr int SMEM_BYTES = BAR_OFF + 64 + 1024;
 };
-
-VJ_DEVINL void named_bar_sync_attn(int id, int n) { asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(n) : "memory"); }
 
 // ---------------------------------------------------------------------------------------------
 // delta[h, t] = sum_d dO[t, h*HD + d] * O[t, h*HD + d]
@@ -77,603 +70,178 @@ __global__ void __launch_bounds__(256) attn_delta_kernel(const __nv_bfloat16* __
 }
 
 // ---------------------------------------------------------------------------------------------
-// dK / dV : CTA = (kv tile, sequence, head)
+// DKV = true : CTA = (128-key tile, sequence, head); resident K, V; streamed Q_i, dO_i.  Writes dK, dV.
+// DKV = false: CTA = (128-query tile, sequence, head); resident Q, dO; streamed K_j, V_j.  Writes dQ.
+// The two share the pipeline and the P / dS algebra; only the orientation of the score fragment differs: in the dK/dV
+// kernel the fragment's rows are keys and its columns queries (lse2 / delta are per column), in the dQ kernel the
+// reverse (lse2 / delta per row).
 // ---------------------------------------------------------------------------------------------
-// FUSE_DQ: the CTA also forms dQ_i (partial over this key tile) = dS_i K  - A operand = the dS^T tile read M-major,
-// B = the K tile read MN-major - and reduce-adds it (TMA, fp32) into a global accumulator, which makes the
-// separate dQ kernel (a second exp / S / dP recomputation) unnecessary.
-constexpr int kDkvThreads = 64 + 8 * 32;   // TMA warp, MMA warp, 8 softmax warps
-
-// TA: P^T and dS^T reach the dV / dK MMAs through TENSOR MEMORY (bf16 pairs written in place over the S^T / dP^T columns each
-// softmax warp has just read, A operand of tcgen05.mma) instead of a [128 x 128] bf16 shared-memory tile.  The kernel is
-// shared-memory-bandwidth bound (ncu, profiles/r02_ncu_attn_bwd1_hd32.txt: LSU shared wavefronts 61 % + tensor-core
-// operand wavefronts 40 % of the data pipe): this removes the P store, and the two 32 KB A-operand reads per tile.  Only
-// the fused dQ MMA still needs dS^T in shared memory (M-major A); tcgen05.mma executes in issue order, so dV (reads P^T) is
-// issued before dP^T (overwrites it) and dK (reads dS^T) before the next S^T.
-template <int HD, bool FUSE_DQ, bool TA>
-__global__ void __launch_bounds__(kDkvThreads, HD <= 64 ? 2 : 1)
-attn_bwd_dkv_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_constant__ CUtensorMap tmDO,
-                    const __grid_constant__ CUtensorMap tmDQ, const AttnBwdParams p) {
-  using C = AttnCfg<HD>;
+template <int HD, bool DKV>
+__global__ void __launch_bounds__(kBwdThreads, 1)
+attn_bwd_kernel(const __grid_constant__ CUtensorMap tmRes, const __grid_constant__ CUtensorMap tmStr,
+                const __grid_constant__ CUtensorMap tmDO, const AttnBwdParams p) {
   using B = BwdCfg<HD>;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+
   const int seq = blockIdx.y, head = blockIdx.z;
   const int row_begin = p.cu_seqlens[seq];
   const int len = p.cu_seqlens[seq + 1] - row_begin;
-  const int kv0 = blockIdx.x * 128;
-  if (kv0 >= len) return;
-  const int n_q = (len + 127) / 128;
-
-  uint64_t* bars = reinterpret_cast<uint64_t*>(smem + B::BAR_OFF);
-  constexpr int ST = B::ST;
-  const uint32_t bar_kv = smem_u32(bars + 0), bar_qdo = smem_u32(bars + 1), bar_qdofree = smem_u32(bars + 3);
-  const uint32_t bar_s = smem_u32(bars + 5), bar_p = smem_u32(bars + 6), bar_pvdone = smem_u32(bars + 7);
-  const uint32_t bar_dp = smem_u32(bars + 8), bar_ds = smem_u32(bars + 9), bar_psfree = smem_u32(bars + 10);
-  const uint32_t bar_stat = smem_u32(bars + 11), bar_statfree = smem_u32(bars + 13);   // [2] each
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 15);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (threadIdx.x == 0) {
-    mbar_init(bar_kv, 1); mbar_init(bar_s, 1);
-    for (int st = 0; st < 2; ++st) {
-      mbar_init(bar_qdo + 8 * st, 1); mbar_init(bar_qdofree + 8 * st, 1);
-      mbar_init(bar_stat + 8 * st, 1); mbar_init(bar_statfree + 8 * st, 8);
-    }
-    mbar_init(bar_p, 8); mbar_init(bar_pvdone, 1); mbar_init(bar_dp, 1); mbar_init(bar_ds, 8);
-    mbar_init(bar_psfree, 1);
-    fence_mbar_init();
-  }
-  if (warp == 0 && lane == 0) { tma_prefetch_desc(&tmQKV); tma_prefetch_desc(&tmDO); }
-  if (warp == 1) tmem_alloc<B::DKV_TMEM>(smem_u32(tmem_slot));
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  const uint32_t tmem_ST = tmem_base, tmem_dV = tmem_base + 128, tmem_dK = tmem_base + 128 + HD;
-  const uint32_t tmem_dQ = tmem_base + 128 + 2 * HD;   // FUSE_DQ only
-  const uint32_t sK = smem_u32(smem + B::T0), sV = smem_u32(smem + B::T1);
-  const uint32_t sQ = smem_u32(smem + B::T2), sDO = smem_u32(smem + B::T3), sPS = smem_u32(smem + B::PS_OFF);
+  const int t0 = blockIdx.x * 128;   // first resident row (key for DKV, query otherwise)
+  if (t0 >= len) return;
+  const int n_it = (len + kBwdStream - 1) / kBwdStream;
   const int HHD = p.H * HD;
 
-  if (warp == 0) {
-    if (lane == 0) {
-      mbar_expect_tx(bar_kv, 2 * C::TILE_BYTES);
-#pragma unroll
-      for (int b = 0; b < C::NBOX; ++b) {
-        tma_load_2d(sK + b * C::BOX_BYTES, &tmQKV, bar_kv, HHD + head * HD + b * C::BOX_INNER, row_begin + kv0);
-        tma_load_2d(sV + b * C::BOX_BYTES, &tmQKV, bar_kv, 2 * HHD + head * HD + b * C::BOX_INNER, row_begin + kv0);
-      }
-    }
-    const uint32_t stats_w = smem_u32(smem + B::STAT_OFF);
-    auto load_qdo = [&](int i) {   // lane 0: Q_i / dO_i tiles into stage i % ST
-      const int st = i % ST;
-      mbar_wait(bar_qdofree + 8 * st, (uint32_t(i / ST) & 1) ^ 1);
-      mbar_expect_tx(bar_qdo + 8 * st, 2 * C::TILE_BYTES);
-#pragma unroll
-      for (int b = 0; b < C::NBOX; ++b) {
-        tma_load_2d(sQ + st * B::STAGE_BYTES + b * C::BOX_BYTES, &tmQKV, bar_qdo + 8 * st,
-                    head * HD + b * C::BOX_INNER, row_begin + i * 128);
-        tma_load_2d(sDO + st * B::STAGE_BYTES + b * C::BOX_BYTES, &tmDO, bar_qdo + 8 * st,
-                    head * HD + b * C::BOX_INNER, row_begin + i * 128);
-      }
-    };
-    if (lane == 0) load_qdo(0);
-    for (int i = 0; i < n_q; ++i) {
-      // per-query-row softmax statistics of tile i -> smem ring of 2 (keeps the global-load latency off the
-      // softmax warps' chain).  +inf LSE for rows past the sequence end -> ex2(s - inf) = 0: no predicates needed.
-      const int sb = i & 1;
-      if (i >= 2) mbar_wait(bar_statfree + 8 * sb, uint32_t((i >> 1) - 1) & 1);
-      float lv[4], dv[4];
-#pragma unroll
-      for (int k = 0; k < 4; ++k) {   // all 8 loads in flight before the first store
-        const int qrow = i * 128 + k * 32 + lane;
-        const bool ok = qrow < len;
-        const long long g = (long long)head * p.T + row_begin + qrow;
-        lv[k] = ok ? p.lse2[g] : INFINITY;
-        dv[k] = ok ? p.delta[g] : 0.f;
-      }
-#pragma unroll
-      for (int k = 0; k < 4; ++k) {
-        sts32f(stats_w + sb * 1024 + 4 * (k * 32 + lane), lv[k]);
-        sts32f(stats_w + sb * 1024 + 512 + 4 * (k * 32 + lane), dv[k]);
-      }
-      __syncwarp();
-      if (lane == 0) {
-        mbar_arrive(bar_stat + 8 * sb);
-        if (i + 1 < n_q) load_qdo(i + 1);   // may block on the stage being released; the statistics are already out
-      }
-    }
-    __syncwarp();
-  } else if (warp == 1) {
-    if (lane == 0) {
-      constexpr uint32_t idesc_128 = make_idesc_bf16(128, 128, 0, 0);
-      constexpr uint32_t idesc_hd = make_idesc_bf16(128, HD, 0, 1);
-      mbar_wait(bar_kv, 0);
-      // With a double-buffered Q / dO stream (ST == 2) the MMAs are ordered so that the softmax warps never wait
-      // for more than two short MMAs: S^T_{i+1} goes out right after dS_i is published (before the long dK / dQ
-      // MMAs of tile i), and dP^T_i before dV_i.
-      auto issue_S = [&](int i) {
-        const uint32_t sQi = sQ + (i % ST) * B::STAGE_BYTES;
-        mbar_wait(bar_qdo + 8 * (i % ST), uint32_t(i / ST) & 1);
-        tc_fence_after();
-#pragma unroll
-        for (int kk = 0; kk < HD / 16; ++kk)
-          umma_f16(tmem_ST, kmajor_desc<HD>(sK, kk), kmajor_desc<HD>(sQi, kk), idesc_128, kk > 0);
-        umma_commit(bar_s);
-      };
-      for (int i = 0; i < n_q; ++i) {
-        const uint32_t ph = i & 1;
-        const int st = i % ST;
-        const uint32_t sQi = sQ + st * B::STAGE_BYTES, sDOi = sDO + st * B::STAGE_BYTES;
-        if (ST == 1 || i == 0) issue_S(i);    // S^T = K Q_i^T
-        mbar_wait(bar_p, ph);
-        tc_fence_after();
-        if (TA) {
-          // dV += P^T dO_i with P^T read from the S^T columns (queries 0..63 in columns 0..31, 64..127 in 64..95), THEN
-          // dP^T = V dO_i^T over the same columns
-#pragma unroll
-          for (int kk = 0; kk < 8; ++kk)
-            umma_f16_ts(tmem_dV, tmem_ST + (kk >> 2) * 64 + (kk & 3) * 8, mnmajor_desc<HD>(sDOi, kk), idesc_hd, (i > 0 || kk > 0));
-#pragma unroll
-          for (int kk = 0; kk < HD / 16; ++kk)
-            umma_f16(tmem_ST, kmajor_desc<HD>(sV, kk), kmajor_desc<HD>(sDOi, kk), idesc_128, kk > 0);
-          umma_commit(bar_dp);
-        } else {
-          // dP^T = V dO_i^T   (re-uses the S^T columns; all S^T reads are done once bar_p fired)
-#pragma unroll
-          for (int kk = 0; kk < HD / 16; ++kk)
-            umma_f16(tmem_ST, kmajor_desc<HD>(sV, kk), kmajor_desc<HD>(sDOi, kk), idesc_128, kk > 0);
-          umma_commit(bar_dp);
-          // dV += P^T dO_i
-#pragma unroll
-          for (int kk = 0; kk < 8; ++kk)
-            umma_f16(tmem_dV, ptile_desc(sPS, kk), mnmajor_desc<HD>(sDOi, kk), idesc_hd, (i > 0 || kk > 0));
-          umma_commit(bar_pvdone);
-        }
-        mbar_wait(bar_ds, ph);
-        tc_fence_after();
-        if (TA) {
-          // dK += dS^T Q_i (A = dS^T in tensor memory), then the next S^T (it overwrites those columns)
-#pragma unroll
-          for (int kk = 0; kk < 8; ++kk)
-            umma_f16_ts(tmem_dK, tmem_ST + (kk >> 2) * 64 + (kk & 3) * 8, mnmajor_desc<HD>(sQi, kk), idesc_hd, (i > 0 || kk > 0));
-          if (ST == 2 && i + 1 < n_q) issue_S(i + 1);
-        } else {
-          if (ST == 2 && i + 1 < n_q) issue_S(i + 1);
-          // dK += dS^T Q_i
-#pragma unroll
-          for (int kk = 0; kk < 8; ++kk)
-            umma_f16(tmem_dK, ptile_desc(sPS, kk), mnmajor_desc<HD>(sQi, kk), idesc_hd, (i > 0 || kk > 0));
-        }
-        if (FUSE_DQ) {
-          // dQ_i partial [q, hd] = dS_i [q, kv] K [kv, hd]: A = dS^T tile as M-major (q contiguous), B = K MN-major
-          constexpr uint32_t idesc_dq = make_idesc_bf16(128, HD, 1, 1);
-#pragma unroll
-          for (int kk = 0; kk < 8; ++kk)
-            umma_f16(tmem_dQ, make_smem_desc(sPS + kk * 2048, 16384, 1024, 2), mnmajor_desc<HD>(sK, kk), idesc_dq, kk > 0);
-        }
-        umma_commit(bar_qdofree + 8 * st);
-        umma_commit(bar_psfree);
-      }
-    }
-    __syncwarp();
-  } else {
-    // 8 softmax warps: warp (qd, half) owns key rows qd*32.. (its TMEM lane quarter) x query columns half*64..+64.
-    // Two warps per scheduler per CTA (four with the co-resident CTA) hide the ld / MUFU / barrier latencies that a
-    // single warp per scheduler exposes.
-    const int qd = warp & 3;
-    const int half = (warp - 2) >> 2;
-    const int r = qd * 32 + lane;  // key row inside the tile
-    const uint32_t lane_addr = uint32_t(qd * 32) << 16;
-    const uint32_t stats = smem_u32(smem + B::STAT_OFF);
-    const uint32_t ps = sPS;
-    const uint32_t dqs = smem_u32(smem + B::DQS_OFF) + qd * 4096;   // half-0 warps drain the dQ partials
-    const uint32_t kvmask = (!FUSE_DQ || kv0 + r < len) ? 0xFFFFFFFFu : 0u;
-    const bool kv_partial = FUSE_DQ && kv0 + 128 > len;
-    const int col0 = half * 64;
-    auto drain_dq = [&](int qi) {   // dQ partial of query tile qi (lanes = query rows) -> global fp32 accumulator
-      uint32_t v[32];
-      tmem_ld32(tmem_dQ + lane_addr, v);
-      tmem_wait_ld();
-      if (lane == 0) tma_wait_group_read<0>();
-      __syncwarp();
-#pragma unroll
-      for (int j = 0; j < 8; ++j)
-        sts128(dqs + lane * 128 + ((j ^ (lane & 7)) << 4), make_uint4(v[4 * j], v[4 * j + 1], v[4 * j + 2], v[4 * j + 3]));
-      tc_fence_before();
-      fence_proxy_async_smem();
-      __syncwarp();
-      if (lane == 0) {
-        tma_reduce_add_2d(&tmDQ, dqs, head * HD, row_begin + qi * 128 + qd * 32);
-        tma_commit_group();
-      }
-    };
-    for (int i = 0; i < n_q; ++i) {
-      const uint32_t ph = i & 1;
-      const uint32_t lse_s = stats + (i & 1) * 1024 + 4 * col0;
-      const uint32_t del_s = lse_s + 512;
-      mbar_wait(bar_stat + 8 * (i & 1), uint32_t(i >> 1) & 1);
-      mbar_wait(bar_s, ph);
-      tc_fence_after();
-      uint32_t pk[32];
-#pragma unroll
-      for (int c = 0; c < 2; ++c) {
-        uint32_t v[32];
-        tmem_ld32(tmem_ST + lane_addr + col0 + c * 32, v);
-        tmem_wait_ld();
-#pragma unroll
-        for (int e = 0; e < 32; e += 4) {
-          const float4 L = lds128f(lse_s + 4 * (c * 32 + e));
-          const float a0 = ex2_approx(fmaf(__uint_as_float(v[e]), p.scale_log2, -L.x));
-          const float a1 = ex2_approx(fmaf(__uint_as_float(v[e + 1]), p.scale_log2, -L.y));
-          const float a2 = ex2_approx(fmaf(__uint_as_float(v[e + 2]), p.scale_log2, -L.z));
-          const float a3 = ex2_approx(fmaf(__uint_as_float(v[e + 3]), p.scale_log2, -L.w));
-          pk[c * 16 + e / 2] = pack_bf16x2(a0, a1);
-          pk[c * 16 + e / 2 + 1] = pack_bf16x2(a2, a3);
-        }
-        // fused dQ sums over key rows, so rows past the sequence end must carry P = dS = 0; for dK / dV alone they
-        // are merely never stored.  Only the last key tile of a sequence can have such rows.
-        if (kv_partial) {
-#pragma unroll
-          for (int e = 0; e < 16; ++e) pk[c * 16 + e] &= kvmask;
-        }
-        if (TA) {
-          // P^T -> tensor memory, in place: this warp's 64 fp32 score columns start at col0, its 64 bf16 probabilities
-          // take columns col0 .. col0+31 (chunk c -> 16 columns at col0 + 16 c, inside the range chunk 0 has already read)
-          uint32_t lo[16];
-#pragma unroll
-          for (int e = 0; e < 16; ++e) lo[e] = pk[c * 16 + e];
-          tmem_st16(tmem_ST + lane_addr + col0 + c * 16, lo);
-        } else {
-          // the P/dS tile is free once the previous iteration's dK (and dQ) MMAs retired; by then the dQ partial of
-          // tile i-1 is complete as well (drained below)
-          if (c == 0 && i > 0) mbar_wait(bar_psfree, (i - 1) & 1);
-#pragma unroll
-          for (int g = 0; g < 4; ++g)
-            ptile_store(ps, r, half * 8 + c * 4 + g,
-                        make_uint4(pk[c * 16 + 4 * g], pk[c * 16 + 4 * g + 1], pk[c * 16 + 4 * g + 2], pk[c * 16 + 4 * g + 3]));
-        }
-      }
-      if (TA) tmem_wait_st();
-      tc_fence_before();
-      fence_proxy_async_smem();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(bar_p);
-      // TA: the dS^T shared-memory tile (read by the dQ MMA of tile i-1) and the dQ partial of tile i-1 are released by the
-      // same commit; nothing above needed it
-      if (TA && i > 0) mbar_wait(bar_psfree, (i - 1) & 1);
-      // bar_psfree(i-1) was observed above, so the dQ partial of tile i-1 is complete: drain it now, off the MMA
-      // warp's critical path (it is busy with dP^T / dV).
-      if (FUSE_DQ && half == 0 && i > 0) { tc_fence_after(); drain_dq(i - 1); }
-      mbar_wait(bar_dp, ph);
-      tc_fence_after();
-#pragma unroll
-      for (int c = 0; c < 2; ++c) {
-        uint32_t v[32];
-        tmem_ld32(tmem_ST + lane_addr + col0 + c * 32, v);
-        tmem_wait_ld();
-        uint32_t ds[16];
-#pragma unroll
-        for (int e = 0; e < 32; e += 4) {
-          const float4 Dl = lds128f(del_s + 4 * (c * 32 + e));
-          // dS = P o (dP - delta) in packed bf16: the factor is rounded to bf16 like P, one HMUL2 per two elements
-          ds[e / 2] = mul_bf16x2(pk[c * 16 + e / 2],
-                                 pack_bf16x2(__uint_as_float(v[e]) - Dl.x, __uint_as_float(v[e + 1]) - Dl.y));
-          ds[e / 2 + 1] = mul_bf16x2(pk[c * 16 + e / 2 + 1],
-                                     pack_bf16x2(__uint_as_float(v[e + 2]) - Dl.z, __uint_as_float(v[e + 3]) - Dl.w));
-        }
-        if (TA) {
-          if (FUSE_DQ) {   // shared-memory copy for the dQ MMA only (M-major A operand)
-#pragma unroll
-            for (int g = 0; g < 4; ++g)
-              ptile_store(ps, r, half * 8 + c * 4 + g, make_uint4(ds[4 * g], ds[4 * g + 1], ds[4 * g + 2], ds[4 * g + 3]));
-          }
-          tmem_st16(tmem_ST + lane_addr + col0 + c * 16, ds);   // in place over the dP^T columns read so far
-        } else {
-          if (c == 0) mbar_wait(bar_pvdone, ph);  // dV MMA finished reading P^T -> tile may be overwritten with dS^T
-#pragma unroll
-          for (int g = 0; g < 4; ++g)
-            ptile_store(ps, r, half * 8 + c * 4 + g, make_uint4(ds[4 * g], ds[4 * g + 1], ds[4 * g + 2], ds[4 * g + 3]));
-        }
-      }
-      if (TA) tmem_wait_st();
-      tc_fence_before();
-      fence_proxy_async_smem();
-      __syncwarp();
-      if (lane == 0) { mbar_arrive(bar_ds); mbar_arrive(bar_statfree + 8 * (i & 1)); }
-    }
-    // epilogue: half-0 warps store dV, half-1 warps dK (x scale) -> bf16 -> dqkv[:, v / k third], 32 columns at a time
-    mbar_wait(bar_psfree, (n_q - 1) & 1);
-    tc_fence_after();
-    if (FUSE_DQ && half == 0) drain_dq(n_q - 1);
-    const int rows_valid = max(0, min(32, len - kv0 - qd * 32));
-    const uint32_t stage = ps + (warp - 2) * 2048;
-    const uint32_t tmem_src = half == 0 ? tmem_dV : tmem_dK;
-    const float mul = half == 0 ? 1.0f : p.scale;
-    __nv_bfloat16* gbase = p.dqkv + (half == 0 ? 2 : 1) * HHD + head * HD;
-#pragma unroll 1
-    for (int c = 0; c < HD / 32; ++c) {
-      uint32_t v[32];
-      tmem_ld32(tmem_src + lane_addr + c * 32, v);
-      tmem_wait_ld();
-      float acc[32];
-#pragma unroll
-      for (int e = 0; e < 32; ++e) acc[e] = __uint_as_float(v[e]);
-      store_rows_bf16<32>(stage, acc, mul, lane, gbase + c * 32, 3LL * HHD, row_begin + kv0 + qd * 32, rows_valid);
-    }
-    if (FUSE_DQ && half == 0 && lane == 0) tma_wait_group<0>();
-    tc_fence_before();
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc<B::DKV_TMEM>(tmem_base);
-}
-
-// ---------------------------------------------------------------------------------------------
-// dQ : CTA = (query tile, sequence, head)
-// ---------------------------------------------------------------------------------------------
-template <int HD>
-__global__ void __launch_bounds__(kAttnThreads, HD <= 64 ? 2 : 1)
-attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQKV, const __grid_constant__ CUtensorMap tmDO,
-                   const AttnBwdParams p) {
-  using C = AttnCfg<HD>;
-  using B = BwdCfg<HD>;
-  extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  const int seq = blockIdx.y, head = blockIdx.z;
-  const int row_begin = p.cu_seqlens[seq];
-  const int len = p.cu_seqlens[seq + 1] - row_begin;
-  const int q0 = blockIdx.x * 128;
-  if (q0 >= len) return;
-  const int n_kv = (len + 127) / 128;
-
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + B::BAR_OFF);
-  constexpr int ST = B::ST;
-  const uint32_t bar_qdo = smem_u32(bars + 0), bar_kv = smem_u32(bars + 1), bar_kvfree = smem_u32(bars + 3);
-  const uint32_t bar_s = smem_u32(bars + 5), bar_sread = smem_u32(bars + 6), bar_dp = smem_u32(bars + 7);
-  const uint32_t bar_ds = smem_u32(bars + 8), bar_dsfree = smem_u32(bars + 9);
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 12);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const uint32_t bar_res = smem_u32(bars + 0);
+  const uint32_t bar_s0 = smem_u32(bars + 1);   // 2 stages
+  const uint32_t sT0 = smem_u32(smem + B::T0), sT1 = smem_u32(smem + B::T1), sS = smem_u32(smem + B::S_OFF);
+
+  // resident: DKV -> T0 = K, T1 = V;  dQ -> T0 = Q, T1 = dO.   streamed: DKV -> a = Q_i, b = dO_i;  dQ -> a = K_j, b = V_j
+  auto load_stream = [&](int i) {   // thread 0 only
+    const int st = i & 1;
+    const uint32_t a = sS + st * 2 * B::STR, b = a + B::STR, bar = bar_s0 + 8 * st;
+    const int r0 = row_begin + i * kBwdStream;
+    mbar_expect_tx(bar, 2 * B::STR);
+    if (DKV) {
+      attn_load_tile<HD, kBwdStream>(a, &tmStr, bar, head * HD, r0);
+      attn_load_tile<HD, kBwdStream>(b, &tmDO, bar, head * HD, r0);
+    } else {
+      attn_load_tile<HD, kBwdStream>(a, &tmStr, bar, HHD + head * HD, r0);
+      attn_load_tile<HD, kBwdStream>(b, &tmStr, bar, 2 * HHD + head * HD, r0);
+    }
+  };
   if (threadIdx.x == 0) {
-    mbar_init(bar_qdo, 1); mbar_init(bar_s, 1);
-    for (int st = 0; st < 2; ++st) { mbar_init(bar_kv + 8 * st, 1); mbar_init(bar_kvfree + 8 * st, 1); }
-    mbar_init(bar_sread, 4); mbar_init(bar_dp, 1); mbar_init(bar_ds, 4); mbar_init(bar_dsfree, 1);
+    mbar_init(bar_res, 1);
+    mbar_init(bar_s0, 1);
+    mbar_init(bar_s0 + 8, 1);
     fence_mbar_init();
+    mbar_expect_tx(bar_res, 2 * B::RES);
+    if (DKV) {
+      attn_load_tile<HD, 128>(sT0, &tmRes, bar_res, HHD + head * HD, row_begin + t0);
+      attn_load_tile<HD, 128>(sT1, &tmRes, bar_res, 2 * HHD + head * HD, row_begin + t0);
+    } else {
+      attn_load_tile<HD, 128>(sT0, &tmRes, bar_res, head * HD, row_begin + t0);
+      attn_load_tile<HD, 128>(sT1, &tmDO, bar_res, head * HD, row_begin + t0);
+    }
+    load_stream(0);
+    if (n_it > 1) load_stream(1);
   }
-  if (warp == 0 && lane == 0) { tma_prefetch_desc(&tmQKV); tma_prefetch_desc(&tmDO); }
-  if (warp == 1) tmem_alloc<B::DQ_TMEM>(smem_u32(tmem_slot));
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  const uint32_t tmem_S = tmem_base, tmem_dQ = tmem_base + 128;
-  const uint32_t sQ = smem_u32(smem + B::T0), sDO = smem_u32(smem + B::T1);
-  const uint32_t sK = smem_u32(smem + B::T2), sV = smem_u32(smem + B::T3), sDS = smem_u32(smem + B::PS_OFF);
-  const int HHD = p.H * HD;
 
-  if (warp == 0) {
-    if (lane == 0) {
-      mbar_expect_tx(bar_qdo, 2 * C::TILE_BYTES);
+  const int wg = threadIdx.x >> 7;
+  const int lane = threadIdx.x & 31;
+  const int r = wg * 64 + ((threadIdx.x >> 5) & 3) * 16 + (lane >> 2);   // first fragment row in the resident tile
+  const float* lse_h = p.lse2 + (long long)head * p.T + row_begin;
+  const float* del_h = p.delta + (long long)head * p.T + row_begin;
+  float acc0[HD / 2], acc1[HD / 2];   // DKV: dV, dK;  dQ: dQ (acc1 unused)
 #pragma unroll
-      for (int b = 0; b < C::NBOX; ++b) {
-        tma_load_2d(sQ + b * C::BOX_BYTES, &tmQKV, bar_qdo, head * HD + b * C::BOX_INNER, row_begin + q0);
-        tma_load_2d(sDO + b * C::BOX_BYTES, &tmDO, bar_qdo, head * HD + b * C::BOX_INNER, row_begin + q0);
-      }
-      for (int j = 0; j < n_kv; ++j) {
-        const int st = j % ST;
-        const uint32_t u = uint32_t(j / ST) & 1;
-        mbar_wait(bar_kvfree + 8 * st, u ^ 1);
-        mbar_expect_tx(bar_kv + 8 * st, 2 * C::TILE_BYTES);
+  for (int i = 0; i < HD / 2; ++i) { acc0[i] = 0.f; acc1[i] = 0.f; }
+  float row_lse[2], row_del[2];   // dQ kernel: per-row statistics of the resident queries
+  if (!DKV) {
 #pragma unroll
-        for (int b = 0; b < C::NBOX; ++b) {
-          tma_load_2d(sK + st * B::STAGE_BYTES + b * C::BOX_BYTES, &tmQKV, bar_kv + 8 * st,
-                      HHD + head * HD + b * C::BOX_INNER, row_begin + j * 128);
-          tma_load_2d(sV + st * B::STAGE_BYTES + b * C::BOX_BYTES, &tmQKV, bar_kv + 8 * st,
-                      2 * HHD + head * HD + b * C::BOX_INNER, row_begin + j * 128);
+    for (int h = 0; h < 2; ++h) {
+      const int q = t0 + r + 8 * h;
+      row_lse[h] = q < len ? lse_h[q] : 0.f;
+      row_del[h] = q < len ? del_h[q] : 0.f;
+    }
+  }
+
+  mbar_wait(bar_res, 0);
+  for (int i = 0; i < n_it; ++i) {
+    const int st = i & 1;
+    const uint32_t sa = sS + st * 2 * B::STR, sb = sa + B::STR;
+    const int c0 = i * kBwdStream;   // first streamed row (relative to the sequence)
+    mbar_wait(bar_s0 + 8 * st, (i >> 1) & 1);
+    // DKV: x = S^T = K Q_i^T, y = dP^T = V dO_i^T;   dQ: x = S = Q K_j^T, y = dP = dO V_j^T
+    float x[kBwdStream / 2], y[kBwdStream / 2];
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < HD / 16; ++kk)
+      wgmma_ss<kBwdStream, 0, 0>(x, attn_kmajor_desc<HD, 128>(sT0, wg * 64, kk), attn_kmajor_desc<HD, kBwdStream>(sa, 0, kk),
+                                 kk > 0);
+#pragma unroll
+    for (int kk = 0; kk < HD / 16; ++kk)
+      wgmma_ss<kBwdStream, 0, 0>(y, attn_kmajor_desc<HD, 128>(sT1, wg * 64, kk), attn_kmajor_desc<HD, kBwdStream>(sb, 0, kk),
+                                 kk > 0);
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_regs(x);
+    wgmma_fence_regs(y);
+
+    // x <- P (or P^T), y <- dS (or dS^T);  fragment element [4c + 2h + e]: row r + 8h, column 8c + 2(lane % 4) + e
+#pragma unroll
+    for (int c = 0; c < kBwdStream / 8; ++c)
+#pragma unroll
+      for (int e = 0; e < 2; ++e) {
+        const int col = c0 + 8 * c + 2 * (lane & 3) + e;
+        const bool col_ok = col < len;
+        float cl = 0.f, cd = 0.f;
+        if (DKV && col_ok) { cl = lse_h[col]; cd = del_h[col]; }
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const float l2 = DKV ? cl : row_lse[h], dl = DKV ? cd : row_del[h];
+          float& pv = x[4 * c + 2 * h + e];
+          float& dv = y[4 * c + 2 * h + e];
+          pv = col_ok ? ex2_approx(fmaf(pv, p.scale_log2, -l2)) : 0.f;
+          dv = pv * (dv - dl);
         }
       }
-    }
-    __syncwarp();
-  } else if (warp == 1) {
-    if (lane == 0) {
-      constexpr uint32_t idesc_128 = make_idesc_bf16(128, 128, 0, 0);
-      constexpr uint32_t idesc_hd = make_idesc_bf16(128, HD, 0, 1);
-      mbar_wait(bar_qdo, 0);
-      for (int j = 0; j < n_kv; ++j) {
-        const uint32_t ph = j & 1;
-        const int st = j % ST;
-        const uint32_t sKj = sK + st * B::STAGE_BYTES, sVj = sV + st * B::STAGE_BYTES;
-        mbar_wait(bar_kv + 8 * st, uint32_t(j / ST) & 1);
-        tc_fence_after();
+
+    // DKV: dV += P^T dO_i, dK += dS^T Q_i;   dQ: dQ += dS K_j   (streamed operand read MN-major)
+    wgmma_fence_regs(acc0);
+    wgmma_fence_regs(acc1);
+    wgmma_fence();
 #pragma unroll
-        for (int kk = 0; kk < HD / 16; ++kk)
-          umma_f16(tmem_S, kmajor_desc<HD>(sQ, kk), kmajor_desc<HD>(sKj, kk), idesc_128, kk > 0);
-        umma_commit(bar_s);
-        mbar_wait(bar_sread, ph);
-        tc_fence_after();
-#pragma unroll
-        for (int kk = 0; kk < HD / 16; ++kk)
-          umma_f16(tmem_S, kmajor_desc<HD>(sDO, kk), kmajor_desc<HD>(sVj, kk), idesc_128, kk > 0);
-        umma_commit(bar_dp);
-        mbar_wait(bar_ds, ph);
-        tc_fence_after();
-#pragma unroll
-        for (int kk = 0; kk < 8; ++kk)
-          umma_f16(tmem_dQ, ptile_desc(sDS, kk), mnmajor_desc<HD>(sKj, kk), idesc_hd, (j > 0 || kk > 0));
-        umma_commit(bar_kvfree + 8 * st);
-        umma_commit(bar_dsfree);
+    for (int kk = 0; kk < kBwdStream / 16; ++kk) {
+      uint32_t a[4];
+      if (DKV) {
+        acc_to_afrag(x, kk, a);
+        wgmma_rs<HD, 1>(acc0, a, attn_mnmajor_desc<HD, kBwdStream>(sb, kk), 1);
+        acc_to_afrag(y, kk, a);
+        wgmma_rs<HD, 1>(acc1, a, attn_mnmajor_desc<HD, kBwdStream>(sa, kk), 1);
+      } else {
+        acc_to_afrag(y, kk, a);
+        wgmma_rs<HD, 1>(acc0, a, attn_mnmajor_desc<HD, kBwdStream>(sa, kk), 1);
       }
     }
-    __syncwarp();
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_regs(acc0);
+    wgmma_fence_regs(acc1);
+    __syncthreads();   // both warpgroups are done with stage st
+    if (threadIdx.x == 0 && i + 2 < n_it) load_stream(i + 2);
+  }
+
+  __nv_bfloat16* rows = p.dqkv + (long long)(row_begin + t0) * 3 * HHD + head * HD;
+  if (DKV) {
+    store_frag_bf16<HD>(acc1, p.scale, rows + HHD, 3LL * HHD, r, len - t0);       // dK
+    store_frag_bf16<HD>(acc0, 1.0f, rows + 2 * HHD, 3LL * HHD, r, len - t0);      // dV
   } else {
-    const int qd = warp & 3;
-    const int r = qd * 32 + lane;
-    const uint32_t lane_addr = uint32_t(qd * 32) << 16;
-    const uint32_t dsb = sDS;
-    const bool row_ok = q0 + r < len;
-    const float lse_r = row_ok ? p.lse2[(long long)head * p.T + row_begin + q0 + r] : INFINITY;  // -> P row = 0
-    const float del_r = row_ok ? p.delta[(long long)head * p.T + row_begin + q0 + r] : 0.f;
-    for (int j = 0; j < n_kv; ++j) {
-      const uint32_t ph = j & 1;
-      const int valid = min(128, len - j * 128);
-      mbar_wait(bar_s, ph);
-      tc_fence_after();
-      uint32_t pk[64];
-#pragma unroll
-      for (int c = 0; c < 4; ++c) {
-        uint32_t v[32];
-        tmem_ld32(tmem_S + lane_addr + c * 32, v);
-        tmem_wait_ld();
-        if (valid == 128) {
-#pragma unroll
-          for (int e = 0; e < 32; e += 2) {
-            const float a = ex2_approx(fmaf(__uint_as_float(v[e]), p.scale_log2, -lse_r));
-            const float b = ex2_approx(fmaf(__uint_as_float(v[e + 1]), p.scale_log2, -lse_r));
-            pk[c * 16 + e / 2] = pack_bf16x2(a, b);
-          }
-        } else {
-#pragma unroll
-          for (int e = 0; e < 32; e += 2) {
-            const int k0i = c * 32 + e;
-            float a = ex2_approx(fmaf(__uint_as_float(v[e]), p.scale_log2, -lse_r));
-            float b = ex2_approx(fmaf(__uint_as_float(v[e + 1]), p.scale_log2, -lse_r));
-            a = (k0i < valid) ? a : 0.f;
-            b = (k0i + 1 < valid) ? b : 0.f;
-            pk[c * 16 + e / 2] = pack_bf16x2(a, b);
-          }
-        }
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(bar_sread);
-      mbar_wait(bar_dp, ph);
-      if (j > 0) mbar_wait(bar_dsfree, (j - 1) & 1);  // previous dQ MMA done reading the dS tile
-      tc_fence_after();
-#pragma unroll
-      for (int c = 0; c < 4; ++c) {
-        uint32_t v[32];
-        tmem_ld32(tmem_S + lane_addr + c * 32, v);
-        tmem_wait_ld();
-        uint32_t ds[16];
-#pragma unroll
-        for (int e = 0; e < 32; e += 2) {
-          const uint32_t pp = pk[c * 16 + e / 2];
-          const float a = bf16_lo(pp) * (__uint_as_float(v[e]) - del_r);
-          const float b = bf16_hi(pp) * (__uint_as_float(v[e + 1]) - del_r);
-          ds[e / 2] = pack_bf16x2(a, b);
-        }
-#pragma unroll
-        for (int g = 0; g < 4; ++g)
-          ptile_store(dsb, r, c * 4 + g, make_uint4(ds[4 * g], ds[4 * g + 1], ds[4 * g + 2], ds[4 * g + 3]));
-      }
-      tc_fence_before();
-      fence_proxy_async_smem();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(bar_ds);
-    }
-    mbar_wait(bar_dsfree, (n_kv - 1) & 1);
-    tc_fence_after();
-    float acc[HD];
-#pragma unroll
-    for (int c = 0; c < HD / 32; ++c) {
-      uint32_t v[32];
-      tmem_ld32(tmem_dQ + lane_addr + c * 32, v);
-      tmem_wait_ld();
-#pragma unroll
-      for (int e = 0; e < 32; ++e) acc[c * 32 + e] = __uint_as_float(v[e]);
-    }
-    const int rows_valid = max(0, min(32, len - q0 - qd * 32));
-    store_rows_bf16<HD>(dsb + (warp - 2) * (32 * HD * 2), acc, p.scale, lane, p.dqkv + head * HD, 3LL * HHD,
-                        row_begin + q0 + qd * 32, rows_valid);
-    tc_fence_before();
+    store_frag_bf16<HD>(acc0, p.scale, rows, 3LL * HHD, r, len - t0);             // dQ
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc<B::DQ_TMEM>(tmem_base);
-}
-
-// dqkv[:, q third] = bf16(scale * acc)   (acc fp32 [T, H*HD] filled by the fused dK/dV kernel's reduce-adds)
-__global__ void __launch_bounds__(256) attn_dq_convert_kernel(const float4* __restrict__ acc, __nv_bfloat16* __restrict__ dqkv,
-                                                              long long T, int HHD, float scale) {
-  const int v4 = HHD >> 2;
-  const long long total = T * v4;
-  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
-    const long long t = i / v4;
-    const int c = int(i % v4) * 4;
-    const float4 a = acc[i];
-    uint2 o;
-    o.x = pack_bf16x2(a.x * scale, a.y * scale);
-    o.y = pack_bf16x2(a.z * scale, a.w * scale);
-    *reinterpret_cast<uint2*>(dqkv + t * 3 * HHD + c) = o;
-  }
-}
-
-int launch_attn_delta(const void* out, const void* dout, float* delta, int T, int H, int HD, cudaStream_t s) {
-  int g = (T + 7) / 8;
-  const int cap = num_sms() * 8;
-  if (g > cap) g = cap;
-  attn_delta_kernel<<<g, 256, 0, s>>>(reinterpret_cast<const __nv_bfloat16*>(out), reinterpret_cast<const __nv_bfloat16*>(dout),
-                                      delta, T, H, HD);
-  VJ_CUDA(cudaGetLastError());
-  vj::count_launch(1);
-  return 0;
-}
-
-int launch_attn_dq_convert(const float* dq_acc, void* dqkv, long long T, int HHD, float scale, cudaStream_t s) {
-  long long n4 = T * HHD / 4;
-  long long g = (n4 + 255) / 256;
-  if (g > (long long)num_sms() * 16) g = (long long)num_sms() * 16;
-  attn_dq_convert_kernel<<<int(g), 256, 0, s>>>(reinterpret_cast<const float4*>(dq_acc), reinterpret_cast<__nv_bfloat16*>(dqkv), T,
-                                                HHD, scale);
-  VJ_CUDA(cudaGetLastError());
-  vj::count_launch(1);
-  return 0;
-}
-
-// Default (3) = this file's kernels with P^T / dS^T handed to the dV / dK MMAs through tensor memory (template parameter
-// TA; hd 32, S = 1184: 0.605 ms vs 0.626 ms with the shared-memory tile).  VJ_ATTN_BWD=1 selects the shared-memory form for
-// A/B runs.  Built, validated, measured and removed again in round 2 (git history): attn_bwd2.cu, a persistent CTA owning two
-// key tiles with ping-pong softmax groups (1.006 ms), and a "half chain" variant of this kernel whose two 64-query halves had
-// their own barriers and a polling MMA thread (0.663 ms).
-static int attn_bwd_generation() {
-  static int gen = -1;
-  if (gen < 0) {
-    const char* e = getenv("VJ_ATTN_BWD");
-    gen = (e && e[0] == '1') ? 1 : 3;
-  }
-  return gen;
 }
 
 template <int HD>
 static int launch_attn_bwd(const void* qkv, const void* out, const void* dout, const float* lse2, float* delta,
-                           void* dqkv, float* dq_acc, const int* cu, int nseq, int max_len, int H, int T, float scale,
-                           cudaStream_t s) {
+                           void* dqkv, const int* cu, int nseq, int max_len, int H, int T, float scale, cudaStream_t s) {
   using C = AttnCfg<HD>;
   using B = BwdCfg<HD>;
-  CUtensorMap tq, tdo;
-  int rc = make_tmap_2d(&tq, qkv, 0, (uint64_t)3 * H * HD, T, (uint64_t)3 * H * HD * 2, C::BOX_INNER, 128, C::TMAP_SWIZZLE);
+  CUtensorMap tq128, tq64, tdo128, tdo64;
+  const uint64_t W = (uint64_t)3 * H * HD;
+  int rc = make_tmap_2d(&tq128, qkv, 0, W, T, W * 2, C::BOX_INNER, 128, C::TMAP_SWIZZLE);
+  if (!rc) rc = make_tmap_2d(&tq64, qkv, 0, W, T, W * 2, C::BOX_INNER, kBwdStream, C::TMAP_SWIZZLE);
+  if (!rc) rc = make_tmap_2d(&tdo128, dout, 0, (uint64_t)H * HD, T, (uint64_t)H * HD * 2, C::BOX_INNER, 128, C::TMAP_SWIZZLE);
+  if (!rc) rc = make_tmap_2d(&tdo64, dout, 0, (uint64_t)H * HD, T, (uint64_t)H * HD * 2, C::BOX_INNER, kBwdStream,
+                             C::TMAP_SWIZZLE);
   if (rc) return rc;
-  rc = make_tmap_2d(&tdo, dout, 0, (uint64_t)H * HD, T, (uint64_t)H * HD * 2, C::BOX_INNER, 128, C::TMAP_SWIZZLE);
-  if (rc) return rc;
-  const bool ta = attn_bwd_generation() == 3;   // P^T / dS^T through tensor memory
-  void (*kdkv)(const CUtensorMap, const CUtensorMap, const CUtensorMap, const AttnBwdParams) =
-      ta ? attn_bwd_dkv_kernel<HD, false, true> : attn_bwd_dkv_kernel<HD, false, false>;
-  void (*kdkv_fused)(const CUtensorMap, const CUtensorMap, const CUtensorMap, const AttnBwdParams) =
-      ta ? attn_bwd_dkv_kernel<HD, B::CAN_FUSE_DQ, true> : attn_bwd_dkv_kernel<HD, B::CAN_FUSE_DQ, false>;
-  auto kdq = attn_bwd_dq_kernel<HD>;
-  static int configured = -1;
-  if (configured != int(ta)) {
+  auto kdkv = attn_bwd_kernel<HD, true>;
+  auto kdq = attn_bwd_kernel<HD, false>;
+  static bool configured = false;
+  if (!configured) {
     VJ_CUDA(cudaFuncSetAttribute(kdkv, cudaFuncAttributeMaxDynamicSharedMemorySize, B::SMEM_BYTES));
-    VJ_CUDA(cudaFuncSetAttribute(kdkv_fused, cudaFuncAttributeMaxDynamicSharedMemorySize, B::SMEM_BYTES));
     VJ_CUDA(cudaFuncSetAttribute(kdq, cudaFuncAttributeMaxDynamicSharedMemorySize, B::SMEM_BYTES));
-    configured = int(ta);
-  }
-  const bool fuse = B::CAN_FUSE_DQ && dq_acc != nullptr;
-  CUtensorMap tdq = tdo;
-  if (fuse) {
-    VJ_CUDA(cudaMemsetAsync(dq_acc, 0, (size_t)T * H * HD * sizeof(float), s));
-    rc = make_tmap_2d(&tdq, dq_acc, 1, (uint64_t)H * HD, T, (uint64_t)H * HD * 4, 32, 32, 3);
-    if (rc) return rc;
+    configured = true;
   }
   {
     int g = (T + 7) / 8;
@@ -682,29 +250,17 @@ static int launch_attn_bwd(const void* qkv, const void* out, const void* dout, c
     attn_delta_kernel<<<g, 256, 0, s>>>(reinterpret_cast<const __nv_bfloat16*>(out),
                                         reinterpret_cast<const __nv_bfloat16*>(dout), delta, T, H, HD);
     VJ_CUDA(cudaGetLastError());
-  vj::count_launch(1);
+    vj::count_launch(1);
   }
   AttnBwdParams p;
   p.cu_seqlens = cu; p.lse2 = lse2; p.delta = delta; p.dqkv = reinterpret_cast<__nv_bfloat16*>(dqkv);
   p.H = H; p.T = T; p.scale = scale; p.scale_log2 = scale * 1.4426950408889634f;
   dim3 grid((max_len + 127) / 128, nseq, H);
-  if (fuse) {
-    kdkv_fused<<<grid, kDkvThreads, B::SMEM_BYTES, s>>>(tq, tdo, tdq, p);
-    VJ_CUDA(cudaGetLastError());
-    long long n4 = (long long)T * H * HD / 4;
-    long long g = (n4 + 255) / 256;
-    if (g > (long long)num_sms() * 16) g = (long long)num_sms() * 16;
-    attn_dq_convert_kernel<<<int(g), 256, 0, s>>>(reinterpret_cast<const float4*>(dq_acc), p.dqkv, T, H * HD, scale);
-    VJ_CUDA(cudaGetLastError());
-    vj::count_launch(2);
-    return 0;
-  }
-  kdkv<<<grid, kDkvThreads, B::SMEM_BYTES, s>>>(tq, tdo, tdq, p);
+  kdkv<<<grid, kBwdThreads, B::SMEM_BYTES, s>>>(tq128, tq64, tdo64, p);
   VJ_CUDA(cudaGetLastError());
-  vj::count_launch(1);
-  kdq<<<grid, kAttnThreads, B::SMEM_BYTES, s>>>(tq, tdo, p);
+  kdq<<<grid, kBwdThreads, B::SMEM_BYTES, s>>>(tq128, tq64, tdo128, p);
   VJ_CUDA(cudaGetLastError());
-  vj::count_launch(1);
+  vj::count_launch(2);
   return 0;
 }
 
@@ -714,13 +270,14 @@ extern "C" int vj_attn_bwd(const void* qkv, const void* out, const void* dout, c
                            void* dqkv, float* dq_acc_ws, const int* cu_seqlens, int nseq, int max_len, int H, int HD,
                            int T, float scale, void* stream_) {
   using namespace vj;
+  (void)dq_acc_ws;   // unused: dQ always comes from its own kernel (see the header)
   cudaStream_t s = reinterpret_cast<cudaStream_t>(stream_);
   VJ_CHECK_ARG(qkv && out && dout && lse2 && delta_ws && dqkv && cu_seqlens, "vj_attn_bwd: null pointer");
   VJ_CHECK_ARG(nseq > 0 && max_len > 0 && H > 0 && T > 0, "vj_attn_bwd: empty problem");
   switch (HD) {
-    case 32: return launch_attn_bwd<32>(qkv, out, dout, lse2, delta_ws, dqkv, dq_acc_ws, cu_seqlens, nseq, max_len, H, T, scale, s);
-    case 64: return launch_attn_bwd<64>(qkv, out, dout, lse2, delta_ws, dqkv, dq_acc_ws, cu_seqlens, nseq, max_len, H, T, scale, s);
-    case 128: return launch_attn_bwd<128>(qkv, out, dout, lse2, delta_ws, dqkv, dq_acc_ws, cu_seqlens, nseq, max_len, H, T, scale, s);
+    case 32: return launch_attn_bwd<32>(qkv, out, dout, lse2, delta_ws, dqkv, cu_seqlens, nseq, max_len, H, T, scale, s);
+    case 64: return launch_attn_bwd<64>(qkv, out, dout, lse2, delta_ws, dqkv, cu_seqlens, nseq, max_len, H, T, scale, s);
+    case 128: return launch_attn_bwd<128>(qkv, out, dout, lse2, delta_ws, dqkv, cu_seqlens, nseq, max_len, H, T, scale, s);
     default: set_error("vj_attn_bwd: head dim %d unsupported (32/64/128)", HD); return -1;
   }
 }

@@ -1,131 +1,82 @@
-// Shared tile geometry and smem-descriptor helpers of the attention kernels (fwd and bwd).
+// Shared tile geometry and wgmma descriptor helpers of the attention kernels (fwd and bwd).
+//
+// A [ROWS x HD] bf16 tile of q, k, v, o or dO is loaded by TMA as HD / BOX_INNER boxes of [ROWS x BOX_INNER] (128B swizzle
+// for HD >= 64, 64B swizzle for HD = 32), box after box.  The same tile serves as a K-major wgmma operand (reduction over
+// HD: Q K^T, dO V^T) and as an MN-major one (reduction over its rows: P V, dS K, P^T dO, dS^T Q).
 #pragma once
 #include "common.cuh"
+#include "wgmma.cuh"
 
 namespace vj {
-
-constexpr int kAttnThreads = 192;
 
 template <int HD>
 struct AttnCfg {
   static constexpr int BOX_INNER = HD >= 64 ? 64 : HD;          // elements per TMA box row
-  static constexpr int NBOX = HD / BOX_INNER;                    // boxes per [128 x HD] tile
+  static constexpr int NBOX = HD / BOX_INNER;                    // boxes per [ROWS x HD] tile
   static constexpr int ROW_BYTES = BOX_INNER * 2;                // 128 (SW128) or 64 (SW64)
-  static constexpr int BOX_BYTES = 128 * ROW_BYTES;
-  static constexpr int TILE_BYTES = NBOX * BOX_BYTES;            // Q / K / V tile
-  static constexpr int LAYOUT = HD >= 64 ? 2 : 4;                // smem descriptor swizzle type
+  static constexpr int LAYOUT = HD >= 64 ? 1 : 2;                // wgmma descriptor swizzle type
   static constexpr int TMAP_SWIZZLE = HD >= 64 ? 3 : 2;
   static constexpr int SBO = 8 * ROW_BYTES;                      // 8-row group stride
-  static constexpr int MN_KSTEP = 16 * ROW_BYTES;                // 16 reduction rows of an MN-major tile
-  static constexpr int P_BYTES = 128 * 128 * 2;
-  static constexpr int Q_OFF = 0;
-  static constexpr int K_OFF = TILE_BYTES;
-  static constexpr int V_OFF = 2 * TILE_BYTES;
-  static constexpr int P_OFF = 3 * TILE_BYTES;
-  static constexpr int BAR_OFF = P_OFF + P_BYTES;
-  static constexpr int SMEM_BYTES = BAR_OFF + 128 + 1024;
-  static constexpr int TMEM_COLS = (128 + HD) <= 256 ? 256 : 512;
+  template <int ROWS>
+  static constexpr int tile_bytes() { return ROWS * HD * 2; }
 };
 
-
-// K-major operand descriptor for k-step kk (16 elements) of a [128 x HD] tile
-template <int HD>
-VJ_DEVINL uint64_t kmajor_desc(uint32_t tile, int kk) {
+// K-major descriptor (reduction over HD) of k-step kk (16 elements) of a [ROWS x HD] tile, starting at row `row0`
+template <int HD, int ROWS>
+VJ_DEVINL uint64_t attn_kmajor_desc(uint32_t tile, int row0, int kk) {
   using C = AttnCfg<HD>;
   constexpr int steps_per_box = C::BOX_INNER / 16;
-  const uint32_t addr = tile + (kk / steps_per_box) * C::BOX_BYTES + (kk % steps_per_box) * 32;
+  const uint32_t addr = tile + (kk / steps_per_box) * (ROWS * C::ROW_BYTES) + row0 * C::ROW_BYTES + (kk % steps_per_box) * 32;
   return make_smem_desc(addr, 16, C::SBO, C::LAYOUT);
 }
-// MN-major operand descriptor (N = HD contiguous, reduction = rows) for k-step kk (16 rows)
-template <int HD>
-VJ_DEVINL uint64_t mnmajor_desc(uint32_t tile, int kk) {
+// MN-major descriptor (N = HD contiguous, reduction over rows) of k-step kk (16 rows) of a [ROWS x HD] tile
+template <int HD, int ROWS>
+VJ_DEVINL uint64_t attn_mnmajor_desc(uint32_t tile, int kk) {
   using C = AttnCfg<HD>;
-  return make_smem_desc(tile + kk * C::MN_KSTEP, C::BOX_BYTES, C::SBO, C::LAYOUT);
+  return make_smem_desc(tile + kk * 16 * C::ROW_BYTES, ROWS * C::ROW_BYTES, C::SBO, C::LAYOUT);
 }
-// Byte offsets of k-step kk inside a tile (compile-time when kk is an unrolled loop index): the MMA-issuing thread builds
-// one descriptor per operand tile and only ADDS these (>> 4) to its address field - a tcgen05.mma then costs a couple of
-// integer instructions to issue instead of a descriptor construction (a single thread issues every MMA of the CTA).
-template <int HD>
-VJ_DEVINL constexpr uint32_t kmajor_koff(int kk) {
+
+// TMA load of rows [r0, r0 + ROWS) of the HD columns starting at column c0 (one box per BOX_INNER columns)
+template <int HD, int ROWS>
+VJ_DEVINL void attn_load_tile(uint32_t dst, const CUtensorMap* m, uint32_t bar, int c0, int r0) {
   using C = AttnCfg<HD>;
-  return uint32_t((kk / (C::BOX_INNER / 16)) * C::BOX_BYTES + (kk % (C::BOX_INNER / 16)) * 32);
-}
-template <int HD>
-VJ_DEVINL constexpr uint32_t mnmajor_koff(int kk) { return uint32_t(kk * AttnCfg<HD>::MN_KSTEP); }
-template <int HD>
-VJ_DEVINL uint64_t kmajor_base(uint32_t tile) { return make_smem_desc(tile, 16, AttnCfg<HD>::SBO, AttnCfg<HD>::LAYOUT); }
-template <int HD>
-VJ_DEVINL uint64_t mnmajor_base(uint32_t tile) {
-  return make_smem_desc(tile, AttnCfg<HD>::BOX_BYTES, AttnCfg<HD>::SBO, AttnCfg<HD>::LAYOUT);
-}
-VJ_DEVINL uint64_t desc_advance(uint64_t d, uint32_t bytes) { return d + uint64_t(bytes >> 4); }
-
-// P / dS tile: [128 rows x 128 reduction] bf16, K-major, two 128B-swizzled atoms of 64 columns
-VJ_DEVINL uint64_t ptile_desc(uint32_t tile, int kk) {
-  return make_smem_desc(tile + (kk >> 2) * 16384 + (kk & 3) * 32, 16, 1024, 2);
-}
-
-
-// write 8 packed bf16 (16 bytes) of row r, 16-byte column chunk col8 (0..15) into a [128x128] K-major tile
-VJ_DEVINL void ptile_store(uint32_t tile, int r, int col8, const uint4& u) {
-  sts128(tile + (col8 >> 3) * 16384 + r * 128 + (((col8 & 7) ^ (r & 7)) << 4), u);
-}
-
-// coalesced store of a per-warp staged [32 rows x HD] bf16 block to global rows
-template <int HD>
-VJ_DEVINL void store_rows_bf16(uint32_t stage, const float (&vals)[HD], float mul, int lane, __nv_bfloat16* gbase,
-                               long long ld, int row_first, int rows_valid) {
-  constexpr int ORB = HD * 2, CH = ORB / 16, ROWS_PER_IT = 32 / CH;
 #pragma unroll
-  for (int g = 0; g < CH; ++g) {
-    uint4 u;
-    u.x = pack_bf16x2(vals[8 * g + 0] * mul, vals[8 * g + 1] * mul);
-    u.y = pack_bf16x2(vals[8 * g + 2] * mul, vals[8 * g + 3] * mul);
-    u.z = pack_bf16x2(vals[8 * g + 4] * mul, vals[8 * g + 5] * mul);
-    u.w = pack_bf16x2(vals[8 * g + 6] * mul, vals[8 * g + 7] * mul);
-    sts128(stage + lane * ORB + ((g ^ (lane & (CH - 1))) << 4), u);
-  }
-  __syncwarp();
-#pragma unroll
-  for (int it = 0; it < CH; ++it) {
-    const int rr = it * ROWS_PER_IT + lane / CH;
-    const int g = lane % CH;
-    if (rr < rows_valid) {
-      const uint4 u = lds128(stage + rr * ORB + ((g ^ (rr & (CH - 1))) << 4));
-      *reinterpret_cast<uint4*>(reinterpret_cast<uint8_t*>(gbase) + ((long long)(row_first + rr) * ld) * 2 + g * 16) = u;
-    }
-  }
-  __syncwarp();
+  for (int b = 0; b < C::NBOX; ++b) tma_load_2d(dst + b * ROWS * C::ROW_BYTES, m, bar, c0 + b * C::BOX_INNER, r0);
 }
 
+// m64k16 A fragment (registers) of k-step kk from an m64nN fp32 accumulator fragment of the same rows: the accumulator's
+// column pairs 16kk..16kk+15 are exactly the A operand's k pairs, so P / dS never touch shared memory.
+template <int R>
+VJ_DEVINL void acc_to_afrag(const float (&d)[R], int kk, uint32_t (&a)[4]) {
+  a[0] = pack_bf16x2(d[8 * kk + 0], d[8 * kk + 1]);
+  a[1] = pack_bf16x2(d[8 * kk + 2], d[8 * kk + 3]);
+  a[2] = pack_bf16x2(d[8 * kk + 4], d[8 * kk + 5]);
+  a[3] = pack_bf16x2(d[8 * kk + 6], d[8 * kk + 7]);
+}
 
-// 32 scores -> p = 2^(s*scale - moff), packed fp32x2 scale/subtract and row sums, bf16 pairs stored to TMEM four columns
-// (eight probabilities) at a time.  MASK: columns >= valid (absolute index base + i) produce exactly 0.
-// POLY of every 8 exponentials run on the FMA / ALU pipes (ex2_poly) instead of MUFU, the pipe that bounds softmax.
-// Only the 8-column groups G0 <= g < G1 are processed (lets the caller interleave a tcgen05.ld between two halves).
-template <bool MASK, int POLY = 0, int G0 = 0, int G1 = 4>
-VJ_DEVINL void exp_store32(const uint32_t (&sv)[32], int base, int valid, uint64_t scale2, uint64_t nmoff2, uint64_t& lsum,
-                           uint32_t tmem_p) {
+VJ_DEVINL float quad_max(float v) {
+  v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 1));
+  return fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 2));
+}
+VJ_DEVINL float quad_sum(float v) {
+  v += __shfl_xor_sync(0xffffffffu, v, 1);
+  return v + __shfl_xor_sync(0xffffffffu, v, 2);
+}
+
+// Stores an m64nHD fp32 accumulator fragment (times `mul`) as bf16 rows: thread holds rows r and r + 8 of the
+// warpgroup's 64, column pairs 8j + 2(lane % 4).  Rows at or beyond `rows_valid` are skipped.
+template <int HD>
+VJ_DEVINL void store_frag_bf16(const float (&d)[HD / 2], float mul, __nv_bfloat16* base, long long ld, int r, int rows_valid) {
+  const int lane = threadIdx.x & 31;
 #pragma unroll
-  for (int g = G0; g < G1; ++g) {
-    uint32_t o[4];
+  for (int h = 0; h < 2; ++h) {
+    const int row = r + 8 * h;
+    if (row >= rows_valid) continue;
 #pragma unroll
-    for (int k = 0; k < 4; ++k) {
-      const int i = 8 * g + 2 * k;
-      float xa, xb;
-      upk2(fma2(pk2(__uint_as_float(sv[i]), __uint_as_float(sv[i + 1])), scale2, nmoff2), xa, xb);
-      float a = ((i & 7) >= 8 - POLY) ? ex2_poly(xa) : ex2_approx(xa);
-      float b = (((i + 1) & 7) >= 8 - POLY) ? ex2_poly(xb) : ex2_approx(xb);
-      if (MASK) {
-        a = (base + i < valid) ? a : 0.f;
-        b = (base + i + 1 < valid) ? b : 0.f;
-      }
-      lsum = add2(lsum, pk2(a, b));
-      o[k] = pack_bf16x2(a, b);
-    }
-    tmem_st4(tmem_p + g * 4, make_uint4(o[0], o[1], o[2], o[3]));
+    for (int j = 0; j < HD / 8; ++j)
+      *reinterpret_cast<uint32_t*>(base + (long long)row * ld + 8 * j + 2 * (lane & 3)) =
+          pack_bf16x2(d[4 * j + 2 * h] * mul, d[4 * j + 2 * h + 1] * mul);
   }
 }
-
 
 }  // namespace vj

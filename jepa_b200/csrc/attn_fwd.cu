@@ -1,4 +1,4 @@
-// Dense (non-causal) variable-length flash attention forward on tcgen05 / TMEM (sm_100a).
+// Dense (non-causal) variable-length flash attention forward on wgmma (sm_90a).
 //
 // Replaces F.scaled_dot_product_attention at src/models/utils/modules.py:66-69 (the `mask`
 // argument there is ignored - "masked attention" is attention over the gathered token subset,
@@ -8,22 +8,19 @@
 // layout the qkv GEMM epilogue writes), O bf16 [T, H*HD], lse2 fp32 [H, T] (log2 domain:
 // m*scale*log2e + log2(l)).  Sequences are row ranges [cu[s], cu[s+1]).
 //
-// One CTA = one 128-row query tile of one (sequence, head); two CTAs are resident per SM.
-//   warp 0    : TMA producer (Q once; K_j double-buffered, V_j single-buffered tiles of 128 keys)
-//   warp 1    : MMA issuer.  S_{j+1} = Q K_{j+1}^T is issued as soon as the softmax threads have
-//               pulled S_j out of TMEM, so it overlaps their exp work; O += P_j V_j accumulates in
-//               TMEM across the whole KV loop (V consumed MN-major from the tile it was loaded as).
-//   warps 2-5 : one thread per query row.  S_j is read from TMEM ONCE into registers; row max;
-//               p = ex2(s*scale - m) in place; bf16 P_j goes to a 128B-swizzled K-major smem tile.
-//               The running max is only refreshed (and O / l rescaled in TMEM) when it grew by more
-//               than 2^8 ("lazy rescale"), so the O accumulator normally never leaves TMEM until the
-//               final 1/l normalisation.
+// One CTA = one 128-row query tile of one (sequence, head), two warpgroups of 64 query rows each.  K_j / V_j tiles of
+// 128 keys stream through a two-stage TMA ring (thread 0 refills a stage as soon as both warpgroups are done with it).
+// Per tile: S = Q K_j^T (wgmma, both operands in smem), online softmax on the accumulator fragment in registers,
+// O += P V_j with P as the register A operand (no shared-memory round trip) and V_j read MN-major.
 #include <stdlib.h>
 
 #include "attn_common.cuh"
 #include "vjepa_b200.h"
 
 namespace vj {
+
+constexpr int kFwdThreads = 256;
+constexpr int kFwdKV = 128;   // keys per tile
 
 struct AttnFwdParams {
   const int* cu_seqlens;
@@ -37,46 +34,17 @@ struct AttnFwdParams {
 template <int HD>
 struct FwdCfg {
   using A = AttnCfg<HD>;
+  static constexpr int TILE = A::template tile_bytes<128>();
   static constexpr int Q_OFF = 0;
-  static constexpr int K_OFF = A::TILE_BYTES;                // 2 stages
-  static constexpr int V_OFF = 3 * A::TILE_BYTES;
-  static constexpr int P_OFF = 4 * A::TILE_BYTES;
-  static constexpr int BAR_OFF = P_OFF + A::P_BYTES;
-  static constexpr int SMEM_BYTES = BAR_OFF + 128 + 1024;
-  static constexpr int TMEM_COLS = (128 + HD + 64) <= 256 ? 256 : 512;   // S (fp32) | O (fp32) | P (bf16 pairs)
+  static constexpr int K_OFF = TILE;          // 2 stages
+  static constexpr int V_OFF = 3 * TILE;      // 2 stages
+  static constexpr int BAR_OFF = 5 * TILE;
+  static constexpr int SMEM_BYTES = BAR_OFF + 64 + 1024;
 };
 
-// p = 2^(s*scale - moff) for 32 score columns, summed into l, packed to bf16 and handed to `emit(g, uint4)` eight
-// columns at a time (only four packed registers are live); FULL = no tail masking
-template <bool FULL, typename Emit>
-VJ_DEVINL void exp_pack32(const uint32_t (&sv)[32], int base, int valid, float scale_log2, float moff, float& l,
-                          Emit&& emit) {
-  float l0 = 0.f, l1 = 0.f;
-#pragma unroll
-  for (int g = 0; g < 4; ++g) {
-    uint32_t o[4];
-#pragma unroll
-    for (int k = 0; k < 4; ++k) {
-      const int i = 8 * g + 2 * k;
-      float a = ex2_approx(fmaf(__uint_as_float(sv[i]), scale_log2, -moff));
-      float b = ex2_approx(fmaf(__uint_as_float(sv[i + 1]), scale_log2, -moff));
-      if (!FULL) {
-        a = (base + i < valid) ? a : 0.f;
-        b = (base + i + 1 < valid) ? b : 0.f;
-      }
-      l0 += a;
-      l1 += b;
-      o[k] = pack_bf16x2(a, b);
-    }
-    emit(g, make_uint4(o[0], o[1], o[2], o[3]));
-  }
-  l += l0 + l1;
-}
-
 template <int HD>
-__global__ void __launch_bounds__(kAttnThreads, HD <= 64 ? 2 : 1)
+__global__ void __launch_bounds__(kFwdThreads, 1)
 attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQKV, const AttnFwdParams p) {
-  using C = AttnCfg<HD>;
   using F = FwdCfg<HD>;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -86,232 +54,123 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQKV, const AttnFwdParams p
   const int len = p.cu_seqlens[seq + 1] - row_begin;
   const int q0 = blockIdx.x * 128;
   if (q0 >= len) return;
-  const int n_kv = (len + 127) / 128;
+  const int n_kv = (len + kFwdKV - 1) / kFwdKV;
 
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + F::BAR_OFF);
   const uint32_t bar_q = smem_u32(bars + 0);
-  const uint32_t bar_k0 = smem_u32(bars + 1);      // 2 stages: +0, +8
-  const uint32_t bar_kfree0 = smem_u32(bars + 3);  // 2 stages
-  const uint32_t bar_v = smem_u32(bars + 5);
-  const uint32_t bar_vfree = smem_u32(bars + 6);   // also "PV_j retired": P tile reusable, O readable
-  const uint32_t bar_s = smem_u32(bars + 7);
-  const uint32_t bar_sfree = smem_u32(bars + 8);
-  const uint32_t bar_p = smem_u32(bars + 9);
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + 10);
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (threadIdx.x == 0) {
-    mbar_init(bar_q, 1);
-    mbar_init(bar_k0, 1); mbar_init(bar_k0 + 8, 1);
-    mbar_init(bar_kfree0, 1); mbar_init(bar_kfree0 + 8, 1);
-    mbar_init(bar_v, 1); mbar_init(bar_vfree, 1);
-    mbar_init(bar_s, 1); mbar_init(bar_sfree, 4); mbar_init(bar_p, 4);
-    fence_mbar_init();
-  }
-  if (warp == 0 && lane == 0) tma_prefetch_desc(&tmQKV);
-  if (warp == 1) tmem_alloc<F::TMEM_COLS>(smem_u32(tmem_slot));
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
-  const uint32_t tmem_S = tmem_base;
-  const uint32_t tmem_O = tmem_base + 128;
-  const uint32_t tmem_P = tmem_base + 128 + HD;   // P_j as bf16 pairs: the A operand of the PV MMA, never in smem
-
-  const uint32_t sQ = smem_u32(smem + F::Q_OFF), sK = smem_u32(smem + F::K_OFF);
-  const uint32_t sV = smem_u32(smem + F::V_OFF), sP = smem_u32(smem + F::P_OFF);
+  const uint32_t bar_kv0 = smem_u32(bars + 1);   // 2 stages: +0, +8
+  const uint32_t sQ = smem_u32(smem + F::Q_OFF), sK = smem_u32(smem + F::K_OFF), sV = smem_u32(smem + F::V_OFF);
   const int HHD = p.H * HD;
 
-  if (warp == 0) {
-    if (lane == 0) {
-      mbar_expect_tx(bar_q, C::TILE_BYTES);
-#pragma unroll
-      for (int b = 0; b < C::NBOX; ++b)
-        tma_load_2d(sQ + b * C::BOX_BYTES, &tmQKV, bar_q, head * HD + b * C::BOX_INNER, row_begin + q0);
-      for (int j = 0; j < n_kv; ++j) {
-        const int kr = row_begin + j * 128;
-        const int st = j & 1;
-        const uint32_t use = uint32_t(j >> 1) & 1;   // per-stage phase
-        mbar_wait(bar_kfree0 + 8 * st, use ^ 1);
-        mbar_expect_tx(bar_k0 + 8 * st, C::TILE_BYTES);
-#pragma unroll
-        for (int b = 0; b < C::NBOX; ++b)
-          tma_load_2d(sK + st * C::TILE_BYTES + b * C::BOX_BYTES, &tmQKV, bar_k0 + 8 * st,
-                      HHD + head * HD + b * C::BOX_INNER, kr);
-        mbar_wait(bar_vfree, (j & 1) ^ 1);
-        mbar_expect_tx(bar_v, C::TILE_BYTES);
-#pragma unroll
-        for (int b = 0; b < C::NBOX; ++b)
-          tma_load_2d(sV + b * C::BOX_BYTES, &tmQKV, bar_v, 2 * HHD + head * HD + b * C::BOX_INNER, kr);
-      }
-    }
-    __syncwarp();
-  } else if (warp == 1) {
-    if (lane == 0) {
-      constexpr uint32_t idesc_s = make_idesc_bf16(128, 128, 0, 0);
-      constexpr uint32_t idesc_o = make_idesc_bf16(128, HD, 0, 1);
-      auto issue_qk = [&](int j) {
-        const int st = j & 1;
-        mbar_wait(bar_k0 + 8 * st, uint32_t(j >> 1) & 1);
-        tc_fence_after();
-#pragma unroll
-        for (int kk = 0; kk < HD / 16; ++kk)
-          umma_f16(tmem_S, kmajor_desc<HD>(sQ, kk), kmajor_desc<HD>(sK + st * C::TILE_BYTES, kk), idesc_s, kk > 0);
-        umma_commit(bar_kfree0 + 8 * st);
-        umma_commit(bar_s);
-      };
-      mbar_wait(bar_q, 0);
-      issue_qk(0);
-      for (int j = 0; j < n_kv; ++j) {
-        if (j + 1 < n_kv) {
-          mbar_wait(bar_sfree, j & 1);   // S_j has been pulled into registers
-          issue_qk(j + 1);
-        }
-        mbar_wait(bar_p, j & 1);
-        mbar_wait(bar_v, j & 1);
-        tc_fence_after();
-#pragma unroll
-        for (int kk = 0; kk < 8; ++kk)
-          umma_f16_ts(tmem_O, tmem_P + kk * 8, mnmajor_desc<HD>(sV, kk), idesc_o, (j > 0 || kk > 0));
-        umma_commit(bar_vfree);
-      }
-    }
-    __syncwarp();
-  } else {
-    const int qd = warp & 3;                 // TMEM lane quarter
-    const int r = qd * 32 + lane;            // query row inside the tile
-    const uint32_t lane_addr = uint32_t(qd * 32) << 16;
-    float m_ref = -INFINITY;                 // reference max the accumulators are expressed against
-    float l = 0.f;
-    for (int j = 0; j < n_kv; ++j) {
-      const int valid = min(128, len - j * 128);
-      mbar_wait(bar_s, j & 1);
-      tc_fence_after();
-      // ---- S_j -> registers.  Columns 0..95 stay in registers; the last 32 are only scanned for the row max
-      // here and re-read from TMEM right before their exponentials: 128 live score registers + temporaries do not
-      // fit the 168-register budget of 2 CTAs/SM, and a spill costs an L2 round trip (L1 is carved out to smem).
-      uint32_t s0[32], s1[32], s2[32];
-      float mx = -INFINITY;
-      {
-        uint32_t t3[32];
-        tmem_ld32(tmem_S + lane_addr + 0, s0);
-        tmem_ld32(tmem_S + lane_addr + 32, s1);
-        tmem_ld32(tmem_S + lane_addr + 64, s2);
-        tmem_ld32(tmem_S + lane_addr + 96, t3);
-        tmem_wait_ld();
-        if (valid == 128) {
-#pragma unroll
-          for (int i = 0; i < 32; ++i)
-            mx = fmaxf(fmaxf(mx, __uint_as_float(s0[i])),
-                       fmaxf(__uint_as_float(s1[i]), fmaxf(__uint_as_float(s2[i]), __uint_as_float(t3[i]))));
-        } else {
-#pragma unroll
-          for (int i = 0; i < 32; ++i) {
-            if (i < valid) mx = fmaxf(mx, __uint_as_float(s0[i]));
-            if (32 + i < valid) mx = fmaxf(mx, __uint_as_float(s1[i]));
-            if (64 + i < valid) mx = fmaxf(mx, __uint_as_float(s2[i]));
-            if (96 + i < valid) mx = fmaxf(mx, __uint_as_float(t3[i]));
-          }
-        }
-      }
-      // ---- lazy rescale: only move the reference max when it would overflow the 2^8 head-room
-      const bool grow = (mx - m_ref) * p.scale_log2 > 8.0f;   // true on the first block (m_ref = -inf)
-      if (__any_sync(0xffffffffu, grow)) {
-        if (j > 0) {
-          mbar_wait(bar_vfree, (j - 1) & 1);   // PV_{j-1} retired: O is stable
-          tc_fence_after();
-          const float alpha = grow ? ex2_approx((m_ref - mx) * p.scale_log2) : 1.0f;
-#pragma unroll
-          for (int c = 0; c < HD / 16; ++c) {
-            uint32_t o[16];
-            tmem_ld16(tmem_O + lane_addr + c * 16, o);
-            tmem_wait_ld();
-#pragma unroll
-            for (int i = 0; i < 16; ++i) o[i] = __float_as_uint(__uint_as_float(o[i]) * alpha);
-            tmem_st16(tmem_O + lane_addr + c * 16, o);
-          }
-          tmem_wait_st();
-          l *= alpha;
-        }
-        if (grow) m_ref = mx;
-      }
-      const float moff = m_ref * p.scale_log2;
-      // ---- p = 2^(s*scale - m), packed to bf16 pairs; the single P tile is free once PV_{j-1} retired
-      // the single P tile is free once PV_{j-1} retired (long done by now); each 32-column group is exponentiated,
-      // packed and stored right away so only 16 packed registers are live at a time (no spills in this loop).
-      if (j > 0) mbar_wait(bar_vfree, (j - 1) & 1);
-      auto put = [&](int col8, const uint4& u) {   // 8 probabilities (4 bf16 pairs) of this row -> P columns in TMEM
-        tmem_st4(tmem_P + lane_addr + col8 * 4, u);
-      };
-      auto reload_last = [&]() {   // columns 96..127 again (into s0, dead by now), then S_j is handed back to the MMA warp
-        tmem_ld32(tmem_S + lane_addr + 96, s0);
-        tmem_wait_ld();
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(bar_sfree);
-      };
-      if (valid == 128) {
-        exp_pack32<true>(s0, 0, valid, p.scale_log2, moff, l, [&](int g, const uint4& u) { put(g, u); });
-        exp_pack32<true>(s1, 32, valid, p.scale_log2, moff, l, [&](int g, const uint4& u) { put(4 + g, u); });
-        exp_pack32<true>(s2, 64, valid, p.scale_log2, moff, l, [&](int g, const uint4& u) { put(8 + g, u); });
-        reload_last();
-        exp_pack32<true>(s0, 96, valid, p.scale_log2, moff, l, [&](int g, const uint4& u) { put(12 + g, u); });
-      } else {
-        exp_pack32<false>(s0, 0, valid, p.scale_log2, moff, l, [&](int g, const uint4& u) { put(g, u); });
-        exp_pack32<false>(s1, 32, valid, p.scale_log2, moff, l, [&](int g, const uint4& u) { put(4 + g, u); });
-        exp_pack32<false>(s2, 64, valid, p.scale_log2, moff, l, [&](int g, const uint4& u) { put(8 + g, u); });
-        reload_last();
-        exp_pack32<false>(s0, 96, valid, p.scale_log2, moff, l, [&](int g, const uint4& u) { put(12 + g, u); });
-      }
-      tmem_wait_st();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(bar_p);
-    }
-    // ---- epilogue: O / l -> bf16, staged through the (now idle) P tile for coalesced stores
-    mbar_wait(bar_vfree, (n_kv - 1) & 1);
-    tc_fence_after();
-    const float inv = 1.0f / l;
-    const bool row_ok = q0 + r < len;
-    if (row_ok) p.lse2[(long long)head * p.T + row_begin + q0 + r] = m_ref * p.scale_log2 + log2f(l);
-    constexpr int ORB = HD * 2;               // bytes per output row
-    constexpr int CH = ORB / 16;              // 16-byte chunks per row
-    const uint32_t stage = sP + (warp - 2) * (32 * ORB);
-#pragma unroll
-    for (int c = 0; c < HD / 16; ++c) {
-      uint32_t o[16];
-      tmem_ld16(tmem_O + lane_addr + c * 16, o);
-      tmem_wait_ld();
-#pragma unroll
-      for (int h2 = 0; h2 < 2; ++h2) {
-        uint4 u;
-        u.x = pack_bf16x2(__uint_as_float(o[8 * h2 + 0]) * inv, __uint_as_float(o[8 * h2 + 1]) * inv);
-        u.y = pack_bf16x2(__uint_as_float(o[8 * h2 + 2]) * inv, __uint_as_float(o[8 * h2 + 3]) * inv);
-        u.z = pack_bf16x2(__uint_as_float(o[8 * h2 + 4]) * inv, __uint_as_float(o[8 * h2 + 5]) * inv);
-        u.w = pack_bf16x2(__uint_as_float(o[8 * h2 + 6]) * inv, __uint_as_float(o[8 * h2 + 7]) * inv);
-        const int g = 2 * c + h2;
-        sts128(stage + lane * ORB + ((g ^ (lane & (CH - 1))) << 4), u);
-      }
-    }
-    tc_fence_before();
-    __syncwarp();
-    // coalesced write-out: CH lanes cover one row
-    constexpr int ROWS_PER_IT = 32 / CH;
-#pragma unroll
-    for (int it = 0; it < CH; ++it) {
-      const int rr = it * ROWS_PER_IT + lane / CH;
-      const int g = lane % CH;
-      const int grow_ = q0 + qd * 32 + rr;
-      if (grow_ < len) {
-        const uint4 u = lds128(stage + rr * ORB + ((g ^ (rr & (CH - 1))) << 4));
-        *reinterpret_cast<uint4*>(reinterpret_cast<uint8_t*>(p.out) +
-                                  ((long long)(row_begin + grow_) * p.ld_out + head * HD) * 2 + g * 16) = u;
-      }
-    }
+  auto load_kv = [&](int j) {   // thread 0 only
+    const int st = j & 1;
+    mbar_expect_tx(bar_kv0 + 8 * st, 2 * F::TILE);
+    attn_load_tile<HD, 128>(sK + st * F::TILE, &tmQKV, bar_kv0 + 8 * st, HHD + head * HD, row_begin + j * kFwdKV);
+    attn_load_tile<HD, 128>(sV + st * F::TILE, &tmQKV, bar_kv0 + 8 * st, 2 * HHD + head * HD, row_begin + j * kFwdKV);
+  };
+  if (threadIdx.x == 0) {
+    mbar_init(bar_q, 1);
+    mbar_init(bar_kv0, 1);
+    mbar_init(bar_kv0 + 8, 1);
+    fence_mbar_init();
+    tma_prefetch_desc(&tmQKV);
+    mbar_expect_tx(bar_q, F::TILE);
+    attn_load_tile<HD, 128>(sQ, &tmQKV, bar_q, head * HD, row_begin + q0);
+    load_kv(0);
+    if (n_kv > 1) load_kv(1);
   }
-  tc_fence_before();
   __syncthreads();
-  if (warp == 1) tmem_dealloc<F::TMEM_COLS>(tmem_base);
+
+  const int wg = threadIdx.x >> 7;
+  const int lane = threadIdx.x & 31;
+  const int r = wg * 64 + ((threadIdx.x >> 5) & 3) * 16 + (lane >> 2);   // this thread's first row in the tile (+8: second)
+  float o[HD / 2];
+#pragma unroll
+  for (int i = 0; i < HD / 2; ++i) o[i] = 0.f;
+  float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
+
+  mbar_wait(bar_q, 0);
+  for (int j = 0; j < n_kv; ++j) {
+    const int st = j & 1;
+    const int valid = min(kFwdKV, len - j * kFwdKV);
+    mbar_wait(bar_kv0 + 8 * st, (j >> 1) & 1);
+    float s[kFwdKV / 2];
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < HD / 16; ++kk)
+      wgmma_ss<kFwdKV, 0, 0>(s, attn_kmajor_desc<HD, 128>(sQ, wg * 64, kk),
+                             attn_kmajor_desc<HD, 128>(sK + st * F::TILE, 0, kk), kk > 0);
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_regs(s);
+
+    // ---- online softmax on the fragment: s[4c + 2h + e] = row r + 8h, key 8c + 2(lane % 4) + e
+    float alpha[2];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      float mx = -INFINITY;
+#pragma unroll
+      for (int c = 0; c < kFwdKV / 8; ++c)
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int key = 8 * c + 2 * (lane & 3) + e;
+          float& v = s[4 * c + 2 * h + e];
+          if (key >= valid) v = -INFINITY;
+          mx = fmaxf(mx, v);
+        }
+      mx = quad_max(mx);
+      const float m_new = fmaxf(m_run[h], mx);
+      alpha[h] = ex2_approx((m_run[h] - m_new) * p.scale_log2);   // 0 on the first tile (m_run = -inf)
+      m_run[h] = m_new;
+      const float moff = m_new * p.scale_log2;
+      float sum = 0.f;
+#pragma unroll
+      for (int c = 0; c < kFwdKV / 8; ++c)
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          float& v = s[4 * c + 2 * h + e];
+          v = ex2_approx(fmaf(v, p.scale_log2, -moff));
+          sum += v;
+        }
+      l_run[h] = l_run[h] * alpha[h] + sum;   // per-thread partial; the quad is summed once at the end
+    }
+#pragma unroll
+    for (int c = 0; c < HD / 8; ++c) {
+      o[4 * c + 0] *= alpha[0]; o[4 * c + 1] *= alpha[0];
+      o[4 * c + 2] *= alpha[1]; o[4 * c + 3] *= alpha[1];
+    }
+
+    // ---- O += P V_j
+    wgmma_fence_regs(o);
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < kFwdKV / 16; ++kk) {
+      uint32_t a[4];
+      acc_to_afrag(s, kk, a);
+      wgmma_rs<HD, 1>(o, a, attn_mnmajor_desc<HD, 128>(sV + st * F::TILE, kk), 1);
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_regs(o);
+    __syncthreads();   // both warpgroups are done with stage st
+    if (threadIdx.x == 0 && j + 2 < n_kv) load_kv(j + 2);
+  }
+
+  // ---- epilogue: O / l -> bf16, lse2 (log2 domain)
+  float inv[2];
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const float l = quad_sum(l_run[h]);
+    inv[h] = 1.0f / l;
+    const int row = q0 + r + 8 * h;
+    if ((lane & 3) == 0 && row < len) p.lse2[(long long)head * p.T + row_begin + row] = m_run[h] * p.scale_log2 + log2f(l);
+  }
+#pragma unroll
+  for (int c = 0; c < HD / 8; ++c) {
+    o[4 * c + 0] *= inv[0]; o[4 * c + 1] *= inv[0];
+    o[4 * c + 2] *= inv[1]; o[4 * c + 3] *= inv[1];
+  }
+  store_frag_bf16<HD>(o, 1.0f, p.out + (long long)(row_begin + q0) * p.ld_out + head * HD, p.ld_out, r, len - q0);
 }
 
 template <int HD>
@@ -334,30 +193,10 @@ static int launch_attn_fwd(const void* qkv, void* out, float* lse2, const int* c
   p.H = H; p.T = T; p.ld_out = (long long)H * HD;
   p.scale_log2 = scale * 1.4426950408889634f;
   dim3 grid((max_len + 127) / 128, nseq, H);
-  kern<<<grid, kAttnThreads, F::SMEM_BYTES, s>>>(tm, p);
+  kern<<<grid, kFwdThreads, F::SMEM_BYTES, s>>>(tm, p);
   VJ_CUDA(cudaGetLastError());
   vj::count_launch(1);
   return 0;
-}
-
-// Default: attn_fwd4.cu (64-key tiles, small serial CTAs: four per SM at head dims 32 / 64, two at head dim 128).  This
-// file's kernel (one query tile per CTA, 128-key tiles, two / one CTAs per SM) is the first generation, kept for A/B
-// timing: VJ_ATTN_FWD=1 selects it, 4 forces fwd4, 5 = fwd4 with three CTAs per SM.
-// Measured on B200, 16 heads x 32 sequences (tests/native/test_attn fwdbig, profiles/r02_attn_fwd_variants.txt):
-//   hd 64, S = 1568: this kernel 0.560 ms, fwd4 0.474 ms;  hd 32, S = 1184: 0.319 / 0.268 ms;  hd 128: 0.877 / 0.623 ms.
-// Two more organisations were built, validated and measured in round 2 and then removed from the tree (git history):
-// attn_fwd2.cu, a persistent CTA with two query tiles and ping-pong softmax groups (0.685 ms, 0.646 ms free-running), and
-// attn_fwd3.cu, this kernel with eight softmax warps, two threads per query row (0.567 ms).
-template <int HD, int NCTA>
-int launch_attn_fwd4(const void* qkv, void* out, float* lse2, const int* cu, int nseq, int max_len, int H, int T,
-                     float scale, cudaStream_t s);
-static int attn_fwd_generation() {
-  static int gen = -1;
-  if (gen < 0) {
-    const char* e = getenv("VJ_ATTN_FWD");
-    gen = (e && (e[0] == '1' || e[0] == '4' || e[0] == '5')) ? e[0] - '0' : 0;   // 0 = default choice per head dim
-  }
-  return gen;
 }
 
 }  // namespace vj
@@ -370,16 +209,6 @@ extern "C" int vj_attn_fwd(const void* qkv, void* out, float* lse2, const int* c
   VJ_CHECK_ARG(nseq > 0 && max_len > 0 && H > 0 && T > 0, "vj_attn_fwd: empty problem");
   VJ_CHECK_ARG((reinterpret_cast<uintptr_t>(qkv) & 15) == 0 && (reinterpret_cast<uintptr_t>(out) & 15) == 0,
                "vj_attn_fwd: pointers must be 16-byte aligned");
-  if (attn_fwd_generation() == 4 || attn_fwd_generation() == 0) {
-    if (HD == 128)   // two CTAs per SM (S 64 + O 128 of 256 TMEM columns): 0.623 ms vs 0.877 ms for gen 1 at S = 1568
-      return launch_attn_fwd4<128, 2>(qkv, out, lse2, cu_seqlens, nseq, max_len, H, T, scale, s);
-    if (HD == 32) return launch_attn_fwd4<32, 4>(qkv, out, lse2, cu_seqlens, nseq, max_len, H, T, scale, s);
-    if (HD == 64) return launch_attn_fwd4<64, 4>(qkv, out, lse2, cu_seqlens, nseq, max_len, H, T, scale, s);
-  }
-  if (attn_fwd_generation() == 5) {
-    if (HD == 32) return launch_attn_fwd4<32, 3>(qkv, out, lse2, cu_seqlens, nseq, max_len, H, T, scale, s);
-    if (HD == 64) return launch_attn_fwd4<64, 3>(qkv, out, lse2, cu_seqlens, nseq, max_len, H, T, scale, s);
-  }
   switch (HD) {
     case 32: return launch_attn_fwd<32>(qkv, out, lse2, cu_seqlens, nseq, max_len, H, T, scale, s);
     case 64: return launch_attn_fwd<64>(qkv, out, lse2, cu_seqlens, nseq, max_len, H, T, scale, s);

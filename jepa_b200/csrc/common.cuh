@@ -1,5 +1,5 @@
-// Shared device/host helpers for the sm_100a V-JEPA kernels: raw PTX wrappers for
-// mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (alloc / mma / commit / ld) and the
+// Shared device/host helpers for the sm_90a V-JEPA kernels: raw PTX wrappers for
+// mbarrier, TMA (cp.async.bulk.tensor), the wgmma shared-memory descriptor and the
 // host-side CUtensorMap encoder.  No CUTLASS, no libcuda link dependency (the driver
 // entry point is resolved at run time so the library still loads on a GPU-less host).
 #pragma once
@@ -119,95 +119,6 @@ VJ_DEVINL void tma_wait_group() {
   asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory");
 }
 
-// ---------------------------------------------------------------------------------------
-// device: tcgen05 / TMEM
-// ---------------------------------------------------------------------------------------
-template <int NCOLS>
-VJ_DEVINL void tmem_alloc(uint32_t smem_result_addr) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                   smem_result_addr),
-               "n"(NCOLS)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-template <int NCOLS>
-VJ_DEVINL void tmem_dealloc(uint32_t taddr) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(NCOLS)
-               : "memory");
-}
-VJ_DEVINL void tc_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-VJ_DEVINL void tc_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-// D[tmem] (+)= A[smem desc] * B[smem desc]; single CTA, bf16/f16 inputs.
-VJ_DEVINL void umma_f16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc,
-                        uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// D[tmem] (+)= A[tmem] * B[smem desc]: A is read from tensor memory - 128 lanes = M rows, 32-bit columns each holding two
-// consecutive K elements (a K=16 step is 8 columns).  No shared-memory traffic for A.
-VJ_DEVINL void umma_f16_ts(uint32_t tmem_d, uint32_t tmem_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "r"(tmem_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// Arrive on an mbarrier once every previously issued tcgen05.mma of this thread retired.
-VJ_DEVINL void umma_commit(uint32_t bar) {
-  asm volatile(
-      "tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar)
-      : "memory");
-}
-VJ_DEVINL void tmem_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-VJ_DEVINL void tmem_wait_st() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-
-// 32 lanes x 32 consecutive fp32 columns: thread i of the warp receives lane (base_lane+i).
-VJ_DEVINL void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]),
-        "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]),
-        "=r"(r[14]), "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]),
-        "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]),
-        "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-VJ_DEVINL void tmem_ld16(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]),
-        "=r"(r[7]), "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]),
-        "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
-VJ_DEVINL void tmem_st16(uint32_t taddr, const uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};"
-      ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]),
-        "r"(r[8]), "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15])
-      : "memory");
-}
-VJ_DEVINL void tmem_st4(uint32_t taddr, const uint4& v) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x4.b32 [%0], {%1, %2, %3, %4};" ::"r"(taddr), "r"(v.x), "r"(v.y), "r"(v.z),
-               "r"(v.w)
-               : "memory");
-}
-
 // Explicit shared-space accesses on 32-bit smem addresses.  Pointers derived from the manually aligned
 // dynamic-smem base lose their address space in the compiler and degrade to generic LD/ST otherwise.
 VJ_DEVINL void sts128(uint32_t addr, const uint4& v) {
@@ -240,42 +151,19 @@ VJ_DEVINL float ex2_approx(float x) {
   return y;
 }
 
-// 2^x on the FMA / ALU pipes (no MUFU): Cody-Waite split x = n + f, f in [-0.5, 0.5], degree-3 minimax polynomial for 2^f
-// (max relative error 7.5e-5, a twentieth of a bf16 ulp), 2^n added straight into the exponent field.  Softmax at head
-// dims 64 / 32 is bound by the 16 exp/clk/SM MUFU pipe; a fraction of the exponentials is moved here (FA4's trick).
-// Valid for x <= ~120; x below -126 is clamped (result ~1e-38, i.e. 0 after the bf16 rounding).
-VJ_DEVINL float ex2_poly(float x) {
-  x = fmaxf(x, -126.0f);
-  const float t = x + 12582912.0f;                 // 1.5 * 2^23: round(x) sits in the low mantissa bits of t
-  const float f = x - (t - 12582912.0f);
-  float q = fmaf(f, 0.0551716648f, 0.2426111251f);
-  q = fmaf(q, f, 0.6932609677f);
-  q = fmaf(q, f, 0.9999280572f);
-  return __int_as_float(__float_as_int(q) + (__float_as_int(t) << 23));
-}
-
-// Shared-memory matrix descriptor (tcgen05 "version 1").  Offsets in bytes (16B granules).
-// layout_type: 0 none, 2 128B swizzle, 4 64B swizzle, 6 32B swizzle.
+// Shared-memory matrix descriptor of wgmma (sm_90).  Offsets in bytes (16B granules); the tile base must be aligned to
+// the swizzle pattern (1024 B for 128B swizzle) so the base-offset field stays 0.
+// layout_type: 0 none, 1 128B swizzle, 2 64B swizzle, 3 32B swizzle.
+//   K-major, swizzled : LBO unused, SBO = stride between 8-row groups; a K step inside the swizzle atom adds to the address.
+//   MN-major, swizzled: LBO = stride between swizzle-atom-wide MN chunks, SBO = stride between groups of 8 K rows.
 VJ_DEVINL uint64_t make_smem_desc(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes,
                                   uint32_t layout_type) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);
   d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFF) << 16;
   d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= static_cast<uint64_t>(1) << 46;  // descriptor version (Blackwell)
-  d |= static_cast<uint64_t>(layout_type & 7) << 61;
+  d |= static_cast<uint64_t>(layout_type & 3) << 62;
   return d;
-}
-
-// Instruction descriptor, kind::f16, bf16 x bf16 -> fp32, dense.
-__host__ __device__ constexpr uint32_t make_idesc_bf16(int M, int N, int a_mn_major, int b_mn_major) {
-  return (1u << 4)                      // D format  : f32
-         | (1u << 7)                    // A format  : bf16
-         | (1u << 10)                   // B format  : bf16
-         | (uint32_t(a_mn_major) << 15) // A major   : 0 K, 1 MN
-         | (uint32_t(b_mn_major) << 16) // B major
-         | (uint32_t(N >> 3) << 17)     // N / 8
-         | (uint32_t(M >> 4) << 24);    // M / 16
 }
 
 // ---------------------------------------------------------------------------------------
@@ -285,29 +173,6 @@ VJ_DEVINL uint32_t pack_bf16x2(float lo, float hi) {
   __nv_bfloat162 v = __floats2bfloat162_rn(lo, hi);
   return *reinterpret_cast<uint32_t*>(&v);
 }
-// packed fp32x2 arithmetic (FFMA2 / FMUL2 / FADD2, new on sm_100): two lanes per issue slot
-VJ_DEVINL uint64_t pk2(float lo, float hi) {
-  uint64_t r;
-  asm("mov.b64 %0, {%1, %2};" : "=l"(r) : "f"(lo), "f"(hi));
-  return r;
-}
-VJ_DEVINL void upk2(uint64_t v, float& lo, float& hi) { asm("mov.b64 {%0, %1}, %2;" : "=f"(lo), "=f"(hi) : "l"(v)); }
-VJ_DEVINL uint64_t fma2(uint64_t a, uint64_t b, uint64_t c) {
-  uint64_t d;
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(d) : "l"(a), "l"(b), "l"(c));
-  return d;
-}
-VJ_DEVINL uint64_t mul2(uint64_t a, uint64_t b) {
-  uint64_t d;
-  asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-  return d;
-}
-VJ_DEVINL uint64_t add2(uint64_t a, uint64_t b) {
-  uint64_t d;
-  asm("add.rn.f32x2 %0, %1, %2;" : "=l"(d) : "l"(a), "l"(b));
-  return d;
-}
-
 // packed bf16 multiply (HMUL2.BF16): both lanes rounded to nearest even
 VJ_DEVINL uint32_t mul_bf16x2(uint32_t a, uint32_t b) {
   uint32_t d;

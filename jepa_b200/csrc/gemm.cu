@@ -1,16 +1,14 @@
-// tcgen05 GEMM for the V-JEPA hot path (sm_100a only).
+// wgmma GEMM for the V-JEPA hot path (sm_90a).
 //
-//   D[M,N] = epi( alpha * sum_k A[m,k] * B[n,k] )        bf16 operands, fp32 accumulation in TMEM
+//   D[M,N] = epi( alpha * sum_k A[m,k] * B[n,k] )        bf16 operands, fp32 accumulation in registers
 //
-// One persistent CTA per SM, warp-specialised:
-//   warp 0      : TMA producer   (cp.async.bulk.tensor -> 128B-swizzled smem ring, mbarrier tx)
-//   warp 1      : MMA issuer     (one thread issues tcgen05.mma, commits free the smem stages)
-//   warps 2..9  : epilogue       (tcgen05.ld -> bias / GELU / residual / dGELU -> smem -> TMA store)
-// The accumulator is double-buffered in TMEM (2 x BN columns) so tile i's epilogue overlaps tile
-// i+1's main loop.  Operands may be K-major (reduction dim contiguous; nn.Linear forward) or
-// MN-major (reduction dim strided; dgrad reads W[N_out,K_in] as B, wgrad reads dY and X
-// transposed) - the smem descriptors change, not the data in HBM, so no transposes are
-// materialised.  Split-K work items reduce into fp32 D with TMA reduce-add.
+// One persistent CTA per SM, warp-specialised, 3 warpgroups:
+//   warpgroup 0   : TMA producer   (one thread: cp.async.bulk.tensor -> 128B-swizzled smem ring, mbarrier tx)
+//   warpgroups 1-2: consumers      (each owns 64 of the 128 tile rows: wgmma.mma_async m64nBNk16 from the smem ring,
+//                                   then bias / GELU / residual / dGELU straight from the accumulator registers to HBM)
+// Operands may be K-major (reduction dim contiguous; nn.Linear forward) or MN-major (reduction dim strided; dgrad reads
+// W[N_out,K_in] as B, wgrad reads dY and X transposed) - the smem descriptors and wgmma's transpose bits change, not the
+// data in HBM, so no transposes are materialised.  Split-K / stream-K pieces reduce-add into fp32 D.
 //
 // Replaces the cuBLASLt calls behind nn.Linear on the reference path:
 // src/models/utils/modules.py:31-34 (fc1/fc2), :63 (qkv), :76 (proj),
@@ -21,14 +19,18 @@
 
 #include "common.cuh"
 #include "vjepa_b200.h"
+#include "wgmma.cuh"
 
 namespace vj {
 
 constexpr int BM = 128;
 constexpr int BK = 64;
-constexpr int kEpiWarps = 8;
-constexpr int kGemmThreads = 64 + kEpiWarps * 32;
-constexpr int kEpiBufBytes = 4096;
+constexpr int kGemmThreads = 384;
+// Weight-gradient GEMMs (both operands MN-major) reduce over every token of the batch (K up to ~76k).  They accumulate
+// kPromoteKB k-blocks at a time in a fresh register set and add that partial to the running sum with ordinary fp32 adds:
+// the tensor core's own accumulation then only ever spans 256 products (its rounding over a full-length K gave rel-L2
+// 2.2e-5 against fp64 at K = 76032, this keeps the sum at the plain fp32 summation-order level).
+constexpr int kPromoteKB = 4;
 
 struct GemmParams {
   int M, N, K;
@@ -39,43 +41,30 @@ struct GemmParams {
   int epi;
   const void* aux;
   long long ldaux;
-  int aux_f32;
   const int* aux_rowmap;
   int aux_period;
-  int has_auxout;
+  void* aux_out;
+  long long ldauxout;
+  void* D;
+  long long ldd;
   int reduce_add;
   float alpha;
-  unsigned lbo_k, sbo_k, lbo_mn, sbo_mn;   // smem-descriptor strides (bytes) of the K-major / MN-major operand tiles
 };
 
-constexpr int kAuxRing = 3;          // aux tiles (32 x 32 bf16 = 2 KB) in flight per epilogue warp
-constexpr int kAuxTileBytes = 2048;
-
-// AUXRING: the epilogue reads a bf16 aux matrix (residual / saved gelu') through a per-warp ring of TMA loads; the
-// ring's smem is paid for with one or two operand stages (these GEMMs are epilogue-bound, not pipeline-depth-bound).
-template <int BN, bool AUXRING = false>
+template <int BN>
 struct GemmCfg {
   static constexpr int A_BYTES = BM * BK * 2;
   static constexpr int B_BYTES = BN * BK * 2;
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-  static constexpr int STAGES = AUXRING ? (BN == 256 ? 3 : (BN == 128 ? 4 : 6)) : (BN == 256 ? 4 : (BN == 128 ? 6 : 8));
-  static constexpr int EPI_OFF = STAGES * STAGE_BYTES;
-  static constexpr int RING_OFF = EPI_OFF + kEpiWarps * kEpiBufBytes;
-  static constexpr int BIAS_OFF = RING_OFF + (AUXRING ? kEpiWarps * kAuxRing * kAuxTileBytes : 0);
-  static constexpr int BAR_OFF = BIAS_OFF + BN * 4;
-  static constexpr int NBARS = 2 * STAGES + 4 + kEpiWarps * kAuxRing;
-  static constexpr int SMEM_BYTES = BAR_OFF + NBARS * 8 + 16 + 1024;  // +1024 align slack
-  static constexpr int TMEM_COLS = 2 * BN;
+  static constexpr int STAGES = BN == 256 ? 4 : (BN == 128 ? 6 : 8);
+  static constexpr int BAR_OFF = STAGES * STAGE_BYTES;
+  static constexpr int SMEM_BYTES = BAR_OFF + 2 * STAGES * 8 + 1024;  // +1024 align slack
   static_assert(SMEM_BYTES <= 232448, "GEMM shared memory budget exceeded");
 };
 
-VJ_DEVINL uint32_t swz_off(int row, int chunk, bool rows128) {
-  return rows128 ? uint32_t(row * 128 + ((chunk ^ (row & 7)) << 4))
-                 : uint32_t(row * 64 + ((chunk ^ ((row >> 1) & 3)) << 4));
-}
-
-// Work decomposition shared by the three warp roles.  Classic: work item w = blockIdx.x, blockIdx.x + gridDim.x, ...
-// over tiles x split_k.  Stream-K: the CTA walks its contiguous k-block range, one (tile, k-range) piece at a time.
+// Work decomposition shared by the producer and the consumers.  Classic: work item w = blockIdx.x, blockIdx.x +
+// gridDim.x, ... over tiles x split_k.  Stream-K: the CTA walks its contiguous k-block range, one (tile, k-range) piece
+// at a time.
 struct WorkCursor {
   long long cur, end;
 };
@@ -110,10 +99,6 @@ VJ_DEVINL bool work_next(const GemmParams& p, WorkCursor& c, int& t, int& kb0, i
   return true;
 }
 
-VJ_DEVINL void named_bar_sync(int id, int nthreads) {
-  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
-}
-
 // erf via Abramowitz-Stegun 7.1.26 (|err| < 1.5e-7) - far below the bf16 rounding of the result.
 VJ_DEVINL float erf_as(float x) {
   const float ax = fabsf(x);
@@ -126,110 +111,51 @@ VJ_DEVINL float erf_as(float x) {
   const float r = 1.0f - poly * __expf(-ax * ax);
   return copysignf(r, x);
 }
-VJ_DEVINL float gelu_fast(float x) { return 0.5f * x * (1.0f + erf_as(x * 0.70710678118654752f)); }
-VJ_DEVINL float gelu_grad_fast(float x) {
+// Exact-erf GELU and its derivative sharing one erf / exp evaluation:  g = x Phi(x),  d = Phi(x) + x pdf(x)
+VJ_DEVINL float gelu_and_grad(float x, float& d) {
   const float cdf = 0.5f * (1.0f + erf_as(x * 0.70710678118654752f));
   const float pdf = 0.39894228040143268f * __expf(-0.5f * x * x);
-  return fmaf(x, pdf, cdf);
+  d = fmaf(x, pdf, cdf);
+  return x * cdf;
+}
+VJ_DEVINL float gelu_grad_fast(float x) {
+  float d;
+  gelu_and_grad(x, d);
+  return d;
 }
 
-// Exact-erf GELU (and its derivative) for two elements at a time in packed fp32x2 arithmetic - the GELU epilogues are
-// bound by FP issue slots, FFMA2 halves them.  erf via Abramowitz-Stegun 7.1.25 (|err| <= 2.5e-5, two orders below
-// the bf16 rounding of the result); exp(-x^2/2) is shared between erf and the Gaussian pdf of the derivative.
-//   g = x Phi(x),  d = Phi(x) + x pdf(x)   (d only if GRAD)
-template <bool GRAD>
-VJ_DEVINL void gelu_pair(float& x0, float& x1, float& d0, float& d1) {
-  const uint64_t x2 = pk2(x0, x1);
-  const uint64_t one2 = pk2(1.0f, 1.0f), half2 = pk2(0.5f, 0.5f), mhalf2 = pk2(-0.5f, -0.5f);
-  // e = exp(-x^2 / 2) = 2^(-x^2 * 0.5 log2(e))
-  const uint64_t y2 = mul2(mul2(x2, x2), pk2(0.72134752044448170f, 0.72134752044448170f));
-  float y0, y1;
-  upk2(y2, y0, y1);
-  const uint64_t e2 = pk2(ex2_approx(-y0), ex2_approx(-y1));
-  // t = 1 / (1 + p |x| / sqrt(2))
-  const uint64_t ax2 = pk2(fabsf(x0), fabsf(x1));
-  const uint64_t den2 = fma2(ax2, pk2(0.33267253f, 0.33267253f), one2);   // 0.47047 / sqrt(2)
-  float n0, n1;
-  upk2(den2, n0, n1);
-  const uint64_t t2 = pk2(__fdividef(1.0f, n0), __fdividef(1.0f, n1));
-  uint64_t poly2 = fma2(t2, pk2(0.7478556f, 0.7478556f), pk2(-0.0958798f, -0.0958798f));
-  poly2 = fma2(poly2, t2, pk2(0.3480242f, 0.3480242f));
-  poly2 = mul2(poly2, t2);
-  const uint64_t pe2 = mul2(poly2, e2);               // 1 - erf(|x| / sqrt 2)
-  const uint64_t h2 = fma2(pe2, mhalf2, half2);       // 0.5 erf(|x| / sqrt 2)
-  float h0, h1;
-  upk2(h2, h0, h1);
-  const uint64_t cdf2 = add2(pk2(copysignf(h0, x0), copysignf(h1, x1)), half2);
-  if (GRAD) {
-    const uint64_t dd2 = fma2(mul2(x2, pk2(0.39894228040143268f, 0.39894228040143268f)), e2, cdf2);
-    upk2(dd2, d0, d1);
-  } else {
-    d0 = x0; d1 = x1;
-  }
-  upk2(mul2(x2, cdf2), x0, x1);
-}
+VJ_DEVINL void setmaxnreg_dec40() { asm volatile("setmaxnreg.dec.sync.aligned.u32 40;"); }
+VJ_DEVINL void setmaxnreg_inc232() { asm volatile("setmaxnreg.inc.sync.aligned.u32 232;"); }
 
-// EPI is a compile-time epilogue kind so that e.g. the plain / GELU kernels carry none of the aux-tile code
-// (and registers) of the residual / dGELU ones.
-template <int BN, bool A_MN, bool B_MN, bool OUT_F32, int EPI, bool AUX32, bool RING>
+// EPI is a compile-time epilogue kind so that e.g. the plain / GELU kernels carry none of the aux code.
+template <int BN, bool A_MN, bool B_MN, bool OUT_F32, int EPI, bool AUX32>
 __global__ void __launch_bounds__(kGemmThreads, 1)
-gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
-            const __grid_constant__ CUtensorMap tmD, const __grid_constant__ CUtensorMap tmX,
-            const GemmParams p) {
+gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmParams p) {
   constexpr bool kUsesAux = (EPI == VJ_EPI_ADD || EPI == VJ_EPI_DGELU || EPI == VJ_EPI_MUL);
-  constexpr bool kRing = RING;   // bf16 aux through the TMA ring (short-K GEMMs) or through registers (long-K: keeps
-                                 // the full operand pipeline depth, the epilogue is a small fraction there)
-  static_assert(!RING || (kUsesAux && !AUX32), "aux ring needs a bf16 aux epilogue");
-  using Cfg = GemmCfg<BN, kRing>;
+  using Cfg = GemmCfg<BN>;
   constexpr int STAGES = Cfg::STAGES;
   extern __shared__ uint8_t smem_raw[];
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) &
-                                             ~uintptr_t(1023));
-  uint8_t* epi_base = smem + Cfg::EPI_OFF;
-  float* bias_s = reinterpret_cast<float*>(smem + Cfg::BIAS_OFF);
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + Cfg::BAR_OFF);
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(bars + Cfg::NBARS);
-  const uint32_t rbar_base = smem_u32(bars + 2 * STAGES + 4);   // [kEpiWarps][kAuxRing] aux-tile "full" barriers
-
   const uint32_t full0 = smem_u32(bars);
   const uint32_t empty0 = smem_u32(bars + STAGES);
-  const uint32_t tfull0 = smem_u32(bars + 2 * STAGES);
-  const uint32_t tempty0 = smem_u32(bars + 2 * STAGES + 2);
-
-  const int warp = threadIdx.x >> 5;
-  const int lane = threadIdx.x & 31;
+  const int wg = threadIdx.x >> 7;
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(full0 + 8 * s, 1);
-      mbar_init(empty0 + 8 * s, 1);
+      mbar_init(empty0 + 8 * s, 8);   // one arrive per consumer warp
     }
-    for (int a = 0; a < 2; ++a) {
-      mbar_init(tfull0 + 8 * a, 1);
-      mbar_init(tempty0 + 8 * a, kEpiWarps);
-    }
-    if (kRing)
-      for (int i = 0; i < kEpiWarps * kAuxRing; ++i) mbar_init(rbar_base + 8 * i, 1);
     fence_mbar_init();
-  }
-  if (warp == 0 && lane == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
-    tma_prefetch_desc(&tmD);
-    tma_prefetch_desc(&tmX);
   }
-  if (warp == 1) tmem_alloc<Cfg::TMEM_COLS>(smem_u32(tmem_slot));
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
 
-  const int tiles = p.tiles_m * p.tiles_n;
-  const int total = tiles * p.split_k;
-
-  if (warp == 0) {
+  if (wg == 0) {
     // ------------------------------------------------------------------ TMA producer
-    if (lane == 0) {
+    setmaxnreg_dec40();
+    if (threadIdx.x == 0) {
       int stage = 0;
       uint32_t phase = 0;
       WorkCursor wc = work_begin(p);
@@ -263,288 +189,148 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
         }
       }
     }
-    __syncwarp();
-  } else if (warp == 1) {
-    // ------------------------------------------------------------------ MMA issuer
-    if (lane == 0) {
-      constexpr uint32_t idesc = make_idesc_bf16(BM, BN, A_MN ? 1 : 0, B_MN ? 1 : 0);
-      int stage = 0;
-      uint32_t phase = 0;
-      int acc = 0;
-      uint32_t acc_phase = 0;
-      WorkCursor wc = work_begin(p);
-      int t, kb0, kb1;
-      while (work_next(p, wc, t, kb0, kb1)) {
-        mbar_wait(tempty0 + 8 * acc, acc_phase ^ 1);
-        tc_fence_after();
-        const uint32_t tacc = tmem_base + acc * BN;
-        for (int kb = kb0; kb < kb1; ++kb) {
-          mbar_wait(full0 + 8 * stage, phase);
-          tc_fence_after();
-          const uint32_t sa = smem_u32(smem + stage * Cfg::STAGE_BYTES);
-          const uint32_t sb = sa + Cfg::A_BYTES;
-#pragma unroll
-          for (int kk = 0; kk < BK / 16; ++kk) {
-            const uint64_t da = A_MN ? make_smem_desc(sa + kk * 2048, p.lbo_mn, p.sbo_mn, 2)
-                                     : make_smem_desc(sa + kk * 32, p.lbo_k, p.sbo_k, 2);
-            const uint64_t db = B_MN ? make_smem_desc(sb + kk * 2048, p.lbo_mn, p.sbo_mn, 2)
-                                     : make_smem_desc(sb + kk * 32, p.lbo_k, p.sbo_k, 2);
-            umma_f16(tacc, da, db, idesc, (kb > kb0 || kk > 0) ? 1u : 0u);
-          }
-          umma_commit(empty0 + 8 * stage);  // smem stage reusable once these MMAs retire
-          if (++stage == STAGES) {
-            stage = 0;
-            phase ^= 1;
-          }
-        }
-        umma_commit(tfull0 + 8 * acc);  // accumulator complete -> epilogue
-        acc ^= 1;
-        if (acc == 0) acc_phase ^= 1;
-      }
-    }
-    __syncwarp();
-  } else {
-    // ------------------------------------------------------------------ epilogue warps
-    const int ew = warp - 2;
-    const int q = warp & 3;   // TMEM lane quarter this warp may read
-    const int g = ew >> 2;    // which half of the BN columns
-    constexpr int COLS_PER_WARP = BN / 2;
-    constexpr int NCHUNK = COLS_PER_WARP / 32;
-    uint8_t* buf = epi_base + ew * kEpiBufBytes;
-    const uint32_t buf_u32 = smem_u32(buf);
-    const uint32_t bias_u32 = smem_u32(bias_s);
-    const int etid = threadIdx.x - 64;
-    int acc = 0;
-    uint32_t acc_phase = 0;
-    // aux ring (kRing): this warp's aux tiles are consumed in a fixed order (tile by tile, chunk by chunk), so lane 0
-    // keeps kAuxRing TMA loads in flight ahead of the consumer - across tile boundaries - and re-arms a slot as soon
-    // as it has been read.  HBM latency of the aux stream never reaches the accumulator drain.
-    const uint32_t ring_u32 = smem_u32(smem + Cfg::RING_OFF) + ew * (kAuxRing * kAuxTileBytes);
-    const uint32_t rbar0 = rbar_base + 8 * (ew * kAuxRing);
-    long long ring_w = blockIdx.x;   // tile of the next aux chunk to request
-    int ring_c = 0;                  // ... and its chunk index
-    auto ring_issue = [&](int slot) {   // lane 0 only
-      if (ring_w < total) {
-        const int split = int(ring_w / tiles);
-        const int t = int(ring_w - (long long)split * tiles);
-        const int rm0 = (t / p.tiles_n) * BM, rn0 = (t % p.tiles_n) * BN;
-        mbar_expect_tx(rbar0 + 8 * slot, kAuxTileBytes);
-        tma_load_2d(ring_u32 + slot * kAuxTileBytes, &tmX, rbar0 + 8 * slot, rn0 + g * COLS_PER_WARP + ring_c * 32,
-                    rm0 + q * 32);
-        if (++ring_c == NCHUNK) { ring_c = 0; ring_w += gridDim.x; }
-      }
-    };
-    int rslot = 0;
-    uint32_t rphase = 0;
-    if (kRing && lane == 0) {
-#pragma unroll
-      for (int i = 0; i < kAuxRing; ++i) ring_issue(i);
-    }
-
-    WorkCursor wc = work_begin(p);
-    int t, kb0, kb1;
-    while (work_next(p, wc, t, kb0, kb1)) {
-      const int m0 = (t / p.tiles_n) * BM;
-      const int n0 = (t % p.tiles_n) * BN;
-
-      named_bar_sync(1, kEpiWarps * 32);
-      for (int i = etid; i < BN; i += kEpiWarps * 32)   // the bias joins the piece that holds the first k-block of its tile
-        sts32f(bias_u32 + 4 * i, (p.bias != nullptr && kb0 == 0 && n0 + i < p.N) ? p.bias[n0 + i] : 0.0f);
-      named_bar_sync(1, kEpiWarps * 32);
-
-      const int row0 = m0 + q * 32;
-      // aux tile (residual / pos-embed / pre-activation) prefetch: the coalesced global loads of chunk c+1 are in
-      // flight while chunk c is being processed; chunk 0 is issued before we even wait for the accumulator.
-      const bool use_aux = kUsesAux && !kRing;
-      constexpr bool a128 = AUX32;           // aux element type is compile-time: spills here cost an L2 round trip each
-      const int cshift = a128 ? 3 : 2;
-      const int cpr = 1 << cshift;           // 16B chunks per aux row (shifts, not runtime integer divisions)
-      const int rows_per_it = 32 >> cshift;
-      const int ach = lane & (cpr - 1);
-      const int arow = lane >> cshift;
-      constexpr int kAuxIt = (kUsesAux && !kRing) ? (AUX32 ? 8 : 4) : 0;
-      uint4 axv[kAuxIt > 0 ? kAuxIt : 1];
-      auto aux_issue = [&](int c) {
-        const int col0 = g * COLS_PER_WARP + c * 32;
-#pragma unroll
-        for (int it = 0; it < kAuxIt; ++it) {
-          {
-            const int r = it * rows_per_it + arow;
-            const int grow = row0 + r;
-            uint4 val = make_uint4(0, 0, 0, 0);
-            if (grow < p.M) {
-              long long srow = grow;
-              if (p.aux_rowmap != nullptr) srow = p.aux_rowmap[grow];
-              else if (p.aux_period > 0) srow = grow % p.aux_period;
-              const long long ecol = n0 + col0 + ach * (a128 ? 4 : 8);
-              if (ecol < p.N) {
-                const uint8_t* src = reinterpret_cast<const uint8_t*>(p.aux) + (srow * p.ldaux + ecol) * (a128 ? 4 : 2);
-                val = __ldg(reinterpret_cast<const uint4*>(src));
-              }
-            }
-            axv[it] = val;
-          }
-        }
-      };
-      if (use_aux) aux_issue(0);
-
-      mbar_wait(tfull0 + 8 * acc, acc_phase);
-      tc_fence_after();
-
-#pragma unroll 1
-      for (int c = 0; c < NCHUNK; ++c) {
-        const int col0 = g * COLS_PER_WARP + c * 32;
-        uint32_t v[32];
-        tmem_ld32(tmem_base + (uint32_t(q * 32) << 16) + uint32_t(acc * BN + col0), v);
-        tmem_wait_ld();
-        if (c == NCHUNK - 1) {
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(tempty0 + 8 * acc);
-        }
-        float f[32];
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          const float4 b4 = lds128f(bias_u32 + 4 * (col0 + 4 * j));
-          f[4 * j] = fmaf(__uint_as_float(v[4 * j]), p.alpha, b4.x);
-          f[4 * j + 1] = fmaf(__uint_as_float(v[4 * j + 1]), p.alpha, b4.y);
-          f[4 * j + 2] = fmaf(__uint_as_float(v[4 * j + 2]), p.alpha, b4.z);
-          f[4 * j + 3] = fmaf(__uint_as_float(v[4 * j + 3]), p.alpha, b4.w);
-        }
-
-        // Staging: the 4 KB per-warp buffer is one fp32 tile, or two bf16 tiles (bufA = TMA-store source of D,
-        // bufB = aux staging / pre-activation store source).  The wait for the previous chunk's TMA stores to
-        // have READ the buffer is placed as late as possible so it hides behind this chunk's TMEM load + math.
-        const uint32_t bufA = buf_u32, bufB = buf_u32 + 2048;
-        bool waited = false;
-        auto wait_prev_store = [&]() {
-          if (!waited) {
-            if (lane == 0) tma_wait_group_read<0>();
-            __syncwarp();
-            waited = true;
-          }
-        };
-
-        auto apply = [&](float& acc_v, float aux_v) {
-          if (EPI == VJ_EPI_ADD) acc_v += aux_v;
-          else if (EPI == VJ_EPI_MUL) acc_v *= aux_v;
-          else acc_v *= gelu_grad_fast(aux_v);
-        };
-        if (kRing) {
-          // aux tile of this chunk: landed by TMA (64B-swizzled like the D staging tile); each thread streams its own
-          // row straight into the accumulator registers, then lane 0 re-arms the slot with the chunk kAuxRing ahead
-          mbar_wait(rbar0 + 8 * rslot, rphase);
-          const uint32_t abuf = ring_u32 + rslot * kAuxTileBytes;
-#pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            const uint4 x = lds128(abuf + swz_off(lane, j, false));
-            apply(f[8 * j], bf16_lo(x.x)); apply(f[8 * j + 1], bf16_hi(x.x));
-            apply(f[8 * j + 2], bf16_lo(x.y)); apply(f[8 * j + 3], bf16_hi(x.y));
-            apply(f[8 * j + 4], bf16_lo(x.z)); apply(f[8 * j + 5], bf16_hi(x.z));
-            apply(f[8 * j + 6], bf16_lo(x.w)); apply(f[8 * j + 7], bf16_hi(x.w));
-          }
-          __syncwarp();
-          if (lane == 0) ring_issue(rslot);
-          if (++rslot == kAuxRing) { rslot = 0; rphase ^= 1; }
-        } else if (kUsesAux) {
-          // the prefetched aux tile (32 rows x 32 cols) goes through smem so each thread can pick up its own row
-          const uint32_t abuf = (a128 || OUT_F32) ? bufA : bufB;   // bf16 aux next to a bf16 D tile: no TMA ever reads bufB
-          if (a128 || OUT_F32) wait_prev_store();
-#pragma unroll
-          for (int it = 0; it < kAuxIt; ++it)
-            sts128(abuf + swz_off(it * rows_per_it + arow, ach, a128), axv[it]);
-          if (c + 1 < NCHUNK) aux_issue(c + 1);
-          __syncwarp();
-          // each thread streams its own row back out of smem straight into the accumulator registers
-          if (a128) {
-#pragma unroll
-            for (int j = 0; j < 8; ++j) {
-              const float4 x = lds128f(abuf + swz_off(lane, j, true));
-              apply(f[4 * j], x.x); apply(f[4 * j + 1], x.y); apply(f[4 * j + 2], x.z); apply(f[4 * j + 3], x.w);
-            }
-          } else {
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-              const uint4 x = lds128(abuf + swz_off(lane, j, false));
-              apply(f[8 * j], bf16_lo(x.x)); apply(f[8 * j + 1], bf16_hi(x.x));
-              apply(f[8 * j + 2], bf16_lo(x.y)); apply(f[8 * j + 3], bf16_hi(x.y));
-              apply(f[8 * j + 4], bf16_lo(x.z)); apply(f[8 * j + 5], bf16_hi(x.z));
-              apply(f[8 * j + 6], bf16_lo(x.w)); apply(f[8 * j + 7], bf16_hi(x.w));
-            }
-          }
-          __syncwarp();
-        }
-        bool two_stores = false;
-        if (EPI == VJ_EPI_GELU || EPI == VJ_EPI_GELU_GRAD) {
-          // second output (needed by the backward) leaves through bufB, gelu(pre) through bufA, one bulk group:
-          //   VJ_EPI_GELU      : aux_out = pre-activation
-          //   VJ_EPI_GELU_GRAD : aux_out = gelu'(pre) = Phi(pre) + pre * pdf(pre)  (shares the erf with gelu itself, so
-          //                      the backward's epilogue is a plain multiply instead of a second erf / exp evaluation)
-          // (plain 16-byte global stores straight from registers - thread = row - were measured instead of the staged TMA
-          //  stores: 32 rows x 16 B per instruction are partial-sector writes, qkv_pred fell from 1035 to 629 TF/s.)
-          const bool second = p.has_auxout && !OUT_F32;
-          if (second) wait_prev_store();
-#pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            float d[8];
-#pragma unroll
-            for (int e = 0; e < 8; e += 2)
-              gelu_pair<EPI == VJ_EPI_GELU_GRAD>(f[8 * j + e], f[8 * j + e + 1], d[e], d[e + 1]);
-            if (second) {
-              uint4 o;
-              o.x = pack_bf16x2(d[0], d[1]); o.y = pack_bf16x2(d[2], d[3]);
-              o.z = pack_bf16x2(d[4], d[5]); o.w = pack_bf16x2(d[6], d[7]);
-              sts128(bufB + swz_off(lane, j, false), o);
-            }
-          }
-          two_stores = second;
-        }
-
-        wait_prev_store();
-        if (OUT_F32) {
-#pragma unroll
-          for (int j = 0; j < 8; ++j)
-            sts128f(bufA + swz_off(lane, j, true), make_float4(f[4 * j], f[4 * j + 1], f[4 * j + 2], f[4 * j + 3]));
-        } else {
-#pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            uint4 o;
-            o.x = pack_bf16x2(f[8 * j], f[8 * j + 1]);
-            o.y = pack_bf16x2(f[8 * j + 2], f[8 * j + 3]);
-            o.z = pack_bf16x2(f[8 * j + 4], f[8 * j + 5]);
-            o.w = pack_bf16x2(f[8 * j + 6], f[8 * j + 7]);
-            sts128(bufA + swz_off(lane, j, false), o);
-          }
-        }
-        fence_proxy_async_smem();
-        __syncwarp();
-        if (lane == 0) {
-          if (two_stores) tma_store_2d(&tmX, bufB, n0 + col0, row0);
-          if (OUT_F32 && p.reduce_add) tma_reduce_add_2d(&tmD, bufA, n0 + col0, row0);
-          else tma_store_2d(&tmD, bufA, n0 + col0, row0);
-          tma_commit_group();
-        }
-      }
-      acc ^= 1;
-      if (acc == 0) acc_phase ^= 1;
-    }
-    if (lane == 0) tma_wait_group<0>();
-    __syncwarp();
+    return;
   }
 
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc<Cfg::TMEM_COLS>(tmem_base);
+  // -------------------------------------------------------------------- consumers
+  setmaxnreg_inc232();
+  const int cw = wg - 1;                    // which 64-row half of the tile
+  const int warp_in_wg = (threadIdx.x >> 5) & 3;
+  const int lane = threadIdx.x & 31;
+  constexpr bool kPromote = A_MN && B_MN;
+  static_assert(!kPromote || BN <= 128, "promoted accumulation needs two accumulator sets in registers");
+  int stage = 0;
+  uint32_t phase = 0;
+  float acc[BN / 2];
+  float part[kPromote ? BN / 2 : 1];
+  WorkCursor wc = work_begin(p);
+  int t, kb0, kb1;
+  while (work_next(p, wc, t, kb0, kb1)) {
+    const int m0 = (t / p.tiles_n) * BM;
+    const int n0 = (t % p.tiles_n) * BN;
+    if constexpr (kPromote) {
+#pragma unroll
+      for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+    }
+    int prev = -1;
+    for (int kb = kb0; kb < kb1; ++kb) {
+      mbar_wait(full0 + 8 * stage, phase);
+      const uint32_t sa = smem_u32(smem + stage * Cfg::STAGE_BYTES) + cw * 8192;   // this warpgroup's 64 rows
+      const uint32_t sb = smem_u32(smem + stage * Cfg::STAGE_BYTES) + Cfg::A_BYTES;
+      const uint64_t da0 = A_MN ? make_smem_desc(sa, 8192, 1024, 1) : make_smem_desc(sa, 16, 1024, 1);
+      const uint64_t db0 = B_MN ? make_smem_desc(sb, 8192, 1024, 1) : make_smem_desc(sb, 16, 1024, 1);
+      if constexpr (kPromote) {
+        const bool group_first = (kb - kb0) % kPromoteKB == 0;
+        const bool group_last = (kb - kb0) % kPromoteKB == kPromoteKB - 1 || kb + 1 == kb1;
+        wgmma_fence_regs(part);
+        wgmma_fence();
+#pragma unroll
+        for (int kk = 0; kk < BK / 16; ++kk)
+          wgmma_ss<BN, 1, 1>(part, da0 + ((kk * 2048) >> 4), db0 + ((kk * 2048) >> 4), (!group_first || kk > 0) ? 1 : 0);
+        wgmma_commit();
+        if (group_last) {
+          wgmma_wait<0>();
+          wgmma_fence_regs(part);
+#pragma unroll
+          for (int i = 0; i < BN / 2; ++i) acc[i] += part[i];
+        } else {
+          wgmma_wait<1>();
+        }
+      } else {
+        wgmma_fence_regs(acc);
+        wgmma_fence();
+#pragma unroll
+        for (int kk = 0; kk < BK / 16; ++kk) {
+          const uint32_t koa = A_MN ? kk * 2048 : kk * 32, kob = B_MN ? kk * 2048 : kk * 32;
+          wgmma_ss<BN, A_MN ? 1 : 0, B_MN ? 1 : 0>(acc, da0 + (koa >> 4), db0 + (kob >> 4), (kb > kb0 || kk > 0) ? 1 : 0);
+        }
+        wgmma_commit();
+        wgmma_wait<1>();   // the previous k-block's MMAs have retired: its stage may be refilled
+        wgmma_fence_regs(acc);
+      }
+      if (prev >= 0) {
+        __syncwarp();
+        if (lane == 0) mbar_arrive(empty0 + 8 * prev);
+      }
+      prev = stage;
+      if (++stage == STAGES) {
+        stage = 0;
+        phase ^= 1;
+      }
+    }
+    wgmma_wait<0>();
+    wgmma_fence_regs(acc);
+    __syncwarp();
+    if (lane == 0) mbar_arrive(empty0 + 8 * prev);
+
+    // ---- epilogue straight from the accumulator fragment: thread holds rows r0 and r0 + 8, column pairs 8j + 2(lane%4)
+    const bool add_bias = p.bias != nullptr && kb0 == 0;   // the bias joins the piece holding the tile's first k-block
+    const int r0 = m0 + cw * 64 + warp_in_wg * 16 + (lane >> 2);
+    const int cq = n0 + 2 * (lane & 3);
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int row = r0 + 8 * h;
+      if (row >= p.M) continue;
+      long long arow = row;
+      if (kUsesAux && AUX32) {
+        if (p.aux_rowmap != nullptr) arow = p.aux_rowmap[row];
+        else if (p.aux_period > 0) arow = row % p.aux_period;
+      }
+#pragma unroll
+      for (int j = 0; j < BN / 8; ++j) {
+        const int col = cq + 8 * j;
+        float v0 = acc[4 * j + 2 * h] * p.alpha, v1 = acc[4 * j + 2 * h + 1] * p.alpha;
+        if (add_bias) {
+          const float2 b = __ldg(reinterpret_cast<const float2*>(p.bias + col));
+          v0 += b.x;
+          v1 += b.y;
+        }
+        if (kUsesAux) {
+          float x0, x1;
+          if (AUX32) {
+            const float2 x = __ldg(reinterpret_cast<const float2*>(reinterpret_cast<const float*>(p.aux) + arow * p.ldaux + col));
+            x0 = x.x; x1 = x.y;
+          } else {
+            const uint32_t x = __ldg(reinterpret_cast<const unsigned int*>(reinterpret_cast<const __nv_bfloat16*>(p.aux) +
+                                                                             arow * p.ldaux + col));
+            x0 = bf16_lo(x); x1 = bf16_hi(x);
+          }
+          if (EPI == VJ_EPI_ADD) { v0 += x0; v1 += x1; }
+          else if (EPI == VJ_EPI_MUL) { v0 *= x0; v1 *= x1; }
+          else { v0 *= gelu_grad_fast(x0); v1 *= gelu_grad_fast(x1); }
+        }
+        if (EPI == VJ_EPI_GELU || EPI == VJ_EPI_GELU_GRAD) {
+          //   VJ_EPI_GELU      : aux_out = pre-activation
+          //   VJ_EPI_GELU_GRAD : aux_out = gelu'(pre) (the backward's epilogue is then a plain multiply)
+          float d0, d1;
+          const float g0 = gelu_and_grad(v0, d0), g1 = gelu_and_grad(v1, d1);
+          if (p.aux_out != nullptr) {
+            const uint32_t o = EPI == VJ_EPI_GELU ? pack_bf16x2(v0, v1) : pack_bf16x2(d0, d1);
+            *reinterpret_cast<uint32_t*>(reinterpret_cast<__nv_bfloat16*>(p.aux_out) + (long long)row * p.ldauxout + col) = o;
+          }
+          v0 = g0;
+          v1 = g1;
+        }
+        if (OUT_F32) {
+          float2* dst = reinterpret_cast<float2*>(reinterpret_cast<float*>(p.D) + (long long)row * p.ldd + col);
+          if (p.reduce_add) atomicAdd(dst, make_float2(v0, v1));
+          else *dst = make_float2(v0, v1);
+        } else {
+          *reinterpret_cast<uint32_t*>(reinterpret_cast<__nv_bfloat16*>(p.D) + (long long)row * p.ldd + col) =
+              pack_bf16x2(v0, v1);
+        }
+      }
+    }
+  }
 }
 
 // ---------------------------------------------------------------------------------------------
 // host side
 // ---------------------------------------------------------------------------------------------
-template <int BN, bool A_MN, bool B_MN, bool OUT_F32, int EPI, bool AUX32 = false, bool RING = false>
-static int launch_gemm(const CUtensorMap& tA, const CUtensorMap& tB, const CUtensorMap& tD,
-                       const CUtensorMap& tX, const GemmParams& p, cudaStream_t stream) {
-  using Cfg = GemmCfg<BN, RING>;
-  auto kern = gemm_kernel<BN, A_MN, B_MN, OUT_F32, EPI, AUX32, RING>;
+template <int BN, bool A_MN, bool B_MN, bool OUT_F32, int EPI, bool AUX32 = false>
+static int launch_gemm(const CUtensorMap& tA, const CUtensorMap& tB, const GemmParams& p, cudaStream_t stream) {
+  using Cfg = GemmCfg<BN>;
+  auto kern = gemm_kernel<BN, A_MN, B_MN, OUT_F32, EPI, AUX32>;
   static bool configured = false;  // per instantiation
   if (!configured) {
     VJ_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg::SMEM_BYTES));
@@ -556,39 +342,37 @@ static int launch_gemm(const CUtensorMap& tA, const CUtensorMap& tB, const CUten
     const long long total_kb = (long long)p.tiles_m * p.tiles_n * p.kb_total;
     grid = int((total_kb + p.sk_chunk - 1) / p.sk_chunk);
   }
-  kern<<<grid, kGemmThreads, Cfg::SMEM_BYTES, stream>>>(tA, tB, tD, tX, p);
+  kern<<<grid, kGemmThreads, Cfg::SMEM_BYTES, stream>>>(tA, tB, p);
   VJ_CUDA(cudaGetLastError());
   vj::count_launch(1);
   return 0;
 }
 
 template <int BN>
-static int dispatch_major(int a_mn, int b_mn, int out_f32, int epi, const CUtensorMap& tA, const CUtensorMap& tB,
-                          const CUtensorMap& tD, const CUtensorMap& tX, const GemmParams& p, cudaStream_t s) {
+static int dispatch_major(int a_mn, int b_mn, int out_f32, int epi, int aux_f32, const CUtensorMap& tA,
+                          const CUtensorMap& tB, const GemmParams& p, cudaStream_t s) {
   // instantiated combinations = what the V-JEPA step needs (forward Linear: K/K; dgrad: K/MN; wgrad: MN/MN fp32)
-  const bool ring = p.K <= 1024;   // bf16 aux via the TMA ring for short reductions (see gemm_kernel)
   if (!a_mn && !b_mn) {
-    if (epi == VJ_EPI_NONE) return out_f32 ? launch_gemm<BN, false, false, true, VJ_EPI_NONE>(tA, tB, tD, tX, p, s)
-                                           : launch_gemm<BN, false, false, false, VJ_EPI_NONE>(tA, tB, tD, tX, p, s);
+    if (epi == VJ_EPI_NONE) return out_f32 ? launch_gemm<BN, false, false, true, VJ_EPI_NONE>(tA, tB, p, s)
+                                           : launch_gemm<BN, false, false, false, VJ_EPI_NONE>(tA, tB, p, s);
     if (epi == VJ_EPI_ADD) {
-      if (p.aux_f32) return out_f32 ? launch_gemm<BN, false, false, true, VJ_EPI_ADD, true>(tA, tB, tD, tX, p, s)
-                                    : launch_gemm<BN, false, false, false, VJ_EPI_ADD, true>(tA, tB, tD, tX, p, s);
-      if (!out_f32) return ring ? launch_gemm<BN, false, false, false, VJ_EPI_ADD, false, true>(tA, tB, tD, tX, p, s)
-                                : launch_gemm<BN, false, false, false, VJ_EPI_ADD, false, false>(tA, tB, tD, tX, p, s);
+      if (aux_f32) return out_f32 ? launch_gemm<BN, false, false, true, VJ_EPI_ADD, true>(tA, tB, p, s)
+                                  : launch_gemm<BN, false, false, false, VJ_EPI_ADD, true>(tA, tB, p, s);
+      if (!out_f32) return launch_gemm<BN, false, false, false, VJ_EPI_ADD, false>(tA, tB, p, s);
     }
-    if (epi == VJ_EPI_GELU && !out_f32) return launch_gemm<BN, false, false, false, VJ_EPI_GELU>(tA, tB, tD, tX, p, s);
-    if (epi == VJ_EPI_GELU_GRAD && !out_f32) return launch_gemm<BN, false, false, false, VJ_EPI_GELU_GRAD>(tA, tB, tD, tX, p, s);
-    if (epi == VJ_EPI_DGELU && !out_f32 && !p.aux_f32) return launch_gemm<BN, false, false, false, VJ_EPI_DGELU, false, true>(tA, tB, tD, tX, p, s);
+    if (epi == VJ_EPI_GELU && !out_f32) return launch_gemm<BN, false, false, false, VJ_EPI_GELU>(tA, tB, p, s);
+    if (epi == VJ_EPI_GELU_GRAD && !out_f32) return launch_gemm<BN, false, false, false, VJ_EPI_GELU_GRAD>(tA, tB, p, s);
+    if (epi == VJ_EPI_DGELU && !out_f32 && !aux_f32) return launch_gemm<BN, false, false, false, VJ_EPI_DGELU>(tA, tB, p, s);
   } else if (!a_mn && b_mn) {
-    if (epi == VJ_EPI_NONE) return out_f32 ? launch_gemm<BN, false, true, true, VJ_EPI_NONE>(tA, tB, tD, tX, p, s)
-                                           : launch_gemm<BN, false, true, false, VJ_EPI_NONE>(tA, tB, tD, tX, p, s);
-    if (epi == VJ_EPI_DGELU && !out_f32 && !p.aux_f32) return launch_gemm<BN, false, true, false, VJ_EPI_DGELU, false, true>(tA, tB, tD, tX, p, s);
-    if (epi == VJ_EPI_MUL && !out_f32 && !p.aux_f32)
-      return ring ? launch_gemm<BN, false, true, false, VJ_EPI_MUL, false, true>(tA, tB, tD, tX, p, s)
-                  : launch_gemm<BN, false, true, false, VJ_EPI_MUL, false, false>(tA, tB, tD, tX, p, s);
+    if (epi == VJ_EPI_NONE) return out_f32 ? launch_gemm<BN, false, true, true, VJ_EPI_NONE>(tA, tB, p, s)
+                                           : launch_gemm<BN, false, true, false, VJ_EPI_NONE>(tA, tB, p, s);
+    if (epi == VJ_EPI_DGELU && !out_f32 && !aux_f32) return launch_gemm<BN, false, true, false, VJ_EPI_DGELU>(tA, tB, p, s);
+    if (epi == VJ_EPI_MUL && !out_f32 && !aux_f32) return launch_gemm<BN, false, true, false, VJ_EPI_MUL>(tA, tB, p, s);
   } else if (a_mn && b_mn) {
-    if (epi == VJ_EPI_NONE) return out_f32 ? launch_gemm<BN, true, true, true, VJ_EPI_NONE>(tA, tB, tD, tX, p, s)
-                                           : launch_gemm<BN, true, true, false, VJ_EPI_NONE>(tA, tB, tD, tX, p, s);
+    if constexpr (BN <= 128) {
+      if (epi == VJ_EPI_NONE) return out_f32 ? launch_gemm<BN, true, true, true, VJ_EPI_NONE>(tA, tB, p, s)
+                                             : launch_gemm<BN, true, true, false, VJ_EPI_NONE>(tA, tB, p, s);
+    }
   }
   set_error("vj_gemm: combination a_mn=%d b_mn=%d d_f32=%d epi=%d is not instantiated", a_mn, b_mn, out_f32, epi);
   return -1;
@@ -623,14 +407,15 @@ extern "C" int vj_gemm(const void* A, long long lda, int a_mn, const void* B, lo
   }
   if (a_mn) VJ_CHECK_ARG(M % 8 == 0, "vj_gemm: MN-major A needs M %% 8 == 0");
 
-  const int BN = (N % 256 == 0) ? 256 : (N % 128 == 0 ? 128 : 64);
+  // (weight gradients hold two accumulator sets, see kPromoteKB: at most 128 columns per tile)
+  const int BN = (N % 256 == 0 && !(a_mn && b_mn)) ? 256 : (N % 128 == 0 ? 128 : 64);
   GemmParams p;
   p.M = M; p.N = N; p.K = K;
   p.tiles_m = (M + BM - 1) / BM;
   p.tiles_n = N / BN;
   p.kb_total = (K + BK - 1) / BK;
   // split_k < 0: stream-K - the linearised (tile, k-block) space is cut into one equal contiguous range per SM, so no SM
-  // idles in a ragged last wave (the weight-gradient GEMMs have 32..128 output tiles for 148 SMs); every piece reduce-adds
+  // idles in a ragged last wave (the weight-gradient GEMMs have 32..128 output tiles for 132 SMs); every piece reduce-adds
   p.stream_k = 0;
   p.sk_chunk = 0;
   if (split_k < 0) {
@@ -646,13 +431,20 @@ extern "C" int vj_gemm(const void* A, long long lda, int a_mn, const void* B, lo
   p.split_k = (p.kb_total + p.kb_per_split - 1) / p.kb_per_split;
   p.bias = bias;
   p.epi = epi;
-  p.aux = aux; p.ldaux = ldaux; p.aux_f32 = aux_f32; p.aux_rowmap = aux_rowmap; p.aux_period = aux_period;
-  p.has_auxout = ((epi == VJ_EPI_GELU || epi == VJ_EPI_GELU_GRAD) && aux_out != nullptr) ? 1 : 0;
+  p.aux = aux; p.ldaux = ldaux; p.aux_rowmap = aux_rowmap; p.aux_period = aux_period;
+  p.aux_out = (epi == VJ_EPI_GELU || epi == VJ_EPI_GELU_GRAD) ? aux_out : nullptr;
+  p.ldauxout = ldauxout;
+  p.D = D; p.ldd = ldd;
   p.reduce_add = (accumulate || p.split_k > 1 || p.stream_k) ? 1 : 0;
   p.alpha = alpha;
-  p.lbo_k = 16; p.sbo_k = 1024; p.lbo_mn = 8192; p.sbo_mn = 1024;
 
-  CUtensorMap tA, tB, tD, tX;
+  if (p.aux_out != nullptr)
+    VJ_CHECK_ARG((reinterpret_cast<uintptr_t>(aux_out) & 3) == 0 && ldauxout % 2 == 0, "vj_gemm: aux_out misaligned");
+  if ((epi == VJ_EPI_ADD || epi == VJ_EPI_DGELU || epi == VJ_EPI_MUL) && !aux_f32) {
+    VJ_CHECK_ARG(aux_rowmap == nullptr && aux_period == 0, "vj_gemm: row-mapped / periodic aux must be fp32");
+    VJ_CHECK_ARG(p.split_k == 1, "vj_gemm: aux epilogues do not combine with split-K");
+  }
+  CUtensorMap tA, tB;
   int rc;
   if (!a_mn) rc = make_tmap_2d(&tA, A, 0, K, M, lda * 2, 64, 128, 3);
   else       rc = make_tmap_2d(&tA, A, 0, M, K, lda * 2, 64, 64, 3);
@@ -660,24 +452,9 @@ extern "C" int vj_gemm(const void* A, long long lda, int a_mn, const void* B, lo
   if (!b_mn) rc = make_tmap_2d(&tB, B, 0, K, N, ldb * 2, 64, BN, 3);
   else       rc = make_tmap_2d(&tB, B, 0, N, K, ldb * 2, 64, 64, 3);
   if (rc) return rc;
-  rc = make_tmap_2d(&tD, D, d_f32 ? 1 : 0, N, M, ldd * (d_f32 ? 4 : 2), 32, 32, d_f32 ? 3 : 2);
-  if (rc) return rc;
-  if (p.has_auxout) {
-    VJ_CHECK_ARG((reinterpret_cast<uintptr_t>(aux_out) & 15) == 0 && ldauxout % 8 == 0, "vj_gemm: aux_out misaligned");
-    rc = make_tmap_2d(&tX, aux_out, 0, N, M, ldauxout * 2, 32, 32, 2);
-    if (rc) return rc;
-  } else if ((epi == VJ_EPI_ADD || epi == VJ_EPI_DGELU || epi == VJ_EPI_MUL) && !aux_f32) {
-    // bf16 aux [M, N]: read by the epilogue warps through TMA (same 32 x 32 / 64B-swizzle box as the D tile)
-    VJ_CHECK_ARG(aux_rowmap == nullptr && aux_period == 0, "vj_gemm: row-mapped / periodic aux must be fp32");
-    VJ_CHECK_ARG(p.split_k == 1, "vj_gemm: aux epilogues do not combine with split-K");
-    rc = make_tmap_2d(&tX, aux, 0, N, M, ldaux * 2, 32, 32, 2);
-    if (rc) return rc;
-  } else {
-    tX = tD;
-  }
   switch (BN) {
-    case 256: return dispatch_major<256>(a_mn, b_mn, d_f32, epi, tA, tB, tD, tX, p, stream);
-    case 128: return dispatch_major<128>(a_mn, b_mn, d_f32, epi, tA, tB, tD, tX, p, stream);
-    default:  return dispatch_major<64>(a_mn, b_mn, d_f32, epi, tA, tB, tD, tX, p, stream);
+    case 256: return dispatch_major<256>(a_mn, b_mn, d_f32, epi, aux_f32, tA, tB, p, stream);
+    case 128: return dispatch_major<128>(a_mn, b_mn, d_f32, epi, aux_f32, tA, tB, p, stream);
+    default:  return dispatch_major<64>(a_mn, b_mn, d_f32, epi, aux_f32, tA, tB, p, stream);
   }
 }

@@ -1,4 +1,4 @@
-// Segmented single-pass reductions over the FLAT gradient / Adam-moment buffers of a FlatParamStore (sm_100a, HBM-bound).
+// Segmented single-pass reductions over the FLAT gradient / Adam-moment buffers of a FlatParamStore (sm_90a, HBM-bound).
 //
 // Replaces the per-tensor host-synchronising loops of the reference's logging / clipping helpers:
 //   src/utils/logging.py:91-105  grad_logger   : float(torch.norm(p.grad)) for every weight tensor  (~300 syncs / call)

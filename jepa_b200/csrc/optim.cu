@@ -1,5 +1,5 @@
 // Flat-buffer parameter kernels: fp32 -> bf16 shadow cast, head-dim padding of the predictor's
-// qkv/proj weights (hd 24 -> 32 so attention tiles stay tcgen05-shaped), the target-encoder EMA
+// qkv/proj weights (hd 24 -> 32 so attention tiles stay wgmma-shaped), the target-encoder EMA
 // (app/vjepa/train.py:484-487) and a fused AdamW step (torch.optim.AdamW as configured by
 // app/vjepa/utils.py:156-210).  All HBM-bound, 16-byte vectorised, grid = multiple of the SM count.
 #include "common.cuh"

@@ -1,10 +1,10 @@
-"""Forward / backward schedules of the V-JEPA networks on top of the sm_100a kernels.
+"""Forward / backward schedules of the V-JEPA networks on top of the sm_90a kernels.
 
-This is the B200-first replacement for the autograd graph PyTorch builds over
+This is the GPU-first replacement for the autograd graph PyTorch builds over
 src/models/vision_transformer.py:159-195, src/models/predictor.py:174-239 and
 src/models/utils/modules.py:61-120 in the reference: tokens of ALL masks of a step are
 concatenated into one token-major [T, D] matrix (only attention needs the sequence boundaries, via
-cu_seqlens), every Linear is one tcgen05 GEMM launch with its bias / GELU / residual fused in the
+cu_seqlens), every Linear is one wgmma GEMM launch with its bias / GELU / residual fused in the
 epilogue, and the backward is scheduled by hand - dgrad and wgrad GEMMs read the saved activations
 in place (MN-major descriptors, no transposes) and the wgrads reduce straight into a flat fp32
 gradient buffer.
@@ -47,13 +47,12 @@ import os as _os
 _STREAM_K = _os.environ.get("VJ_GEMM_STREAMK", "0") == "1"     # "1": stream-K wgrads instead of the wave-filling split-K
 
 
-def _split_k_for(m_out, n_in, k_tokens, sms=148):
-    """Split-K factor of a weight-gradient GEMM [m_out, n_in] += dY^T X over k_tokens: the output has 18..128 tiles for 148
+def _split_k_for(m_out, n_in, k_tokens, sms=132):
+    """Split-K factor of a weight-gradient GEMM [m_out, n_in] += dY^T X over k_tokens: the output has 18..128 tiles for 132
     SMs, so pick the split whose work-item count fills whole waves best (a mild penalty per split: every piece reduce-adds
-    a full fp32 tile).  Measured on B200 (tests/native/test_gemm perf): qkv wgrad 96 tiles: split 2 -> 972, 3 / stream-K
-    -> 1313 TF/s; predictor fc2 wgrad 18 tiles: split 8 -> 1308, stream-K 593 TF/s (stream-K stays available as
-    split_k = -1 but loses the L2 sharing of the operand tiles between co-scheduled pieces)."""
-    bn = 256 if n_in % 256 == 0 else (128 if n_in % 128 == 0 else 64)
+    a full fp32 tile).  Stream-K stays available as split_k = -1 but loses the L2 sharing of the operand tiles between
+    co-scheduled pieces.  Weight-gradient tiles are at most 128 columns wide (gemm.cu, kPromoteKB)."""
+    bn = 128 if n_in % 128 == 0 else 64
     tiles = ((m_out + 127) // 128) * (n_in // bn)
     kb = (k_tokens + 63) // 64
     best, best_score = 1, -1.0
@@ -171,7 +170,7 @@ def blocks_forward(spec, weights, x, seq, save, tap=None):
 def _wgrad(dy, act, grad_out, bias_grad, tokens):
     """grad_out[N_out, K_in] += dy^T act ; bias_grad[N_out] += colsum(dy)."""
     n_out, k_in = grad_out.shape
-    # stream-K (split_k = -1): 32..128 output tiles for 148 SMs - every SM gets the same number of k-blocks instead of a
+    # stream-K (split_k = -1): 32..128 output tiles for 132 SMs - every SM gets the same number of k-blocks instead of a
     # ragged second wave; all pieces reduce-add into the flat fp32 gradient buffer anyway
     K.gemm(dy, act, grad_out, a_mn=True, b_mn=True, accumulate=True,
            split_k=-1 if _STREAM_K else _split_k_for(n_out, k_in, tokens))
@@ -196,7 +195,6 @@ def blocks_backward(spec, weights, saved, dx, seq, store, gflat, scratch, sync=N
     H, hd, hdp = spec.heads, spec.hd, spec.hdp
     gv = lambda name: store.grad_view(gflat, name)
     delta_ws = _empty((H * T,), F32, dev)
-    dq_acc_ws = _empty((T, W), F32, dev) if hdp <= 32 else None   # enables the fused dQ path of the attention bwd
     for w, s in zip(reversed(weights), reversed(saved)):
         pre = w.prefix
         # ---- MLP: x_out = x_mid + fc2(gelu(fc1(ln2)))
@@ -213,7 +211,7 @@ def blocks_backward(spec, weights, saved, dx, seq, store, gflat, scratch, sync=N
         dattn = _empty((T, W), BF16, dev)
         K.gemm(dx_mid, w.proj_w, dattn, b_mn=True)
         dqkv = _empty((T, 3 * W), BF16, dev)
-        K.attn_bwd(s.qkv, s.attn, dattn, s.lse, delta_ws, dqkv, cu, nseq, max_len, H, hdp, spec.scale, dq_acc_ws)
+        K.attn_bwd(s.qkv, s.attn, dattn, s.lse, delta_ws, dqkv, cu, nseq, max_len, H, hdp, spec.scale)
         dln1 = _empty((T, D), BF16, dev)
         K.gemm(dqkv, w.qkv_w, dln1, b_mn=True)
         if not spec.padded:

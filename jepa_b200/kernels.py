@@ -1,6 +1,6 @@
 """Tensor-level wrappers over the C ABI: marshal torch CUDA tensors into raw pointers + sizes.
 
-PyTorch is only the allocator / stream provider here; every op below is one of our own sm_100a
+PyTorch is only the allocator / stream provider here; every op below is one of our own sm_90a
 kernels.  All functions enqueue on torch's current stream and never synchronise.
 """
 import torch

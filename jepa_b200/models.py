@@ -1,4 +1,4 @@
-"""Host-side mirror of the reference model API (src/models/*) on top of the sm_100a engine.
+"""Host-side mirror of the reference model API (src/models/*) on top of the sm_90a engine.
 
 Class names, constructor kwargs, parameter names / shapes and state_dict keys follow
 src/models/vision_transformer.py, src/models/predictor.py, src/models/utils/{modules,patch_embed,
@@ -22,7 +22,7 @@ from .tensors import trunc_normal_
 def _require_cuda(t, what):
     if not t.is_cuda:
         raise RuntimeError(
-            f"jepa_b200: {what} needs CUDA tensors - the V-JEPA hot path is implemented only as sm_100a "
+            f"jepa_b200: {what} needs CUDA tensors - the V-JEPA hot path is implemented only as sm_90a "
             "kernels (no CPU or eager-PyTorch fallback).")
 
 
@@ -163,7 +163,7 @@ class _PredictorFn(torch.autograd.Function):
 # VisionTransformer (vision_transformer.py:21-246)
 # -------------------------------------------------------------------------------------------------
 class VisionTransformer(nn.Module):
-    """ Vision Transformer encoder; parameters and API of the reference, math on sm_100a kernels. """
+    """ Vision Transformer encoder; parameters and API of the reference, math on sm_90a kernels. """
 
     def __init__(self, img_size=224, patch_size=16, num_frames=1, tubelet_size=2, in_chans=3, embed_dim=768, depth=12,
                  num_heads=12, mlp_ratio=4.0, qkv_bias=True, qk_scale=None, drop_rate=0.0, attn_drop_rate=0.0,

@@ -3,7 +3,7 @@
 The reference keeps ~300 separate fp32 tensors per network and touches them one by one (autocast
 weight casts, the EMA python loop at app/vjepa/train.py:484-487, foreach AdamW).  Here the
 nn.Parameters of a backbone are re-pointed (``p.data``) into slices of a single buffer so that
-  * the bf16 shadow the tcgen05 GEMMs read is produced by one cast launch per step,
+  * the bf16 shadow the wgmma GEMMs read is produced by one cast launch per step,
   * the target-encoder EMA is one launch,
   * weight gradients are written by the wgrad GEMMs straight into one flat fp32 gradient buffer
     (one NCCL all-reduce region for data parallel).

@@ -1,10 +1,10 @@
-"""Frozen-encoder evaluation side of V-JEPA on the sm_100a kernels (SURVEY section 8, row f4): the attentive probe
+"""Frozen-encoder evaluation side of V-JEPA on the sm_90a kernels (SURVEY section 8, row f4): the attentive probe
 (src/models/attentive_pooler.py:21-136, CrossAttention / CrossAttentionBlock of src/models/utils/modules.py:122-182) and
 the clip aggregation wrapper (evals/video_classification_frozen/utils.py:86-159).
 
 Same constructor arguments, parameter names, initialisation and `state_dict` keys as the reference, so a probe checkpoint
 written by the reference's eval loop loads here unchanged.  The accelerated path is INFERENCE: `forward` runs under
-no-grad on the hand-written kernels (LayerNorm, tcgen05 GEMMs with fused bias / GELU / residual epilogues, and
+no-grad on the hand-written kernels (LayerNorm, wgmma GEMMs with fused bias / GELU / residual epilogues, and
 `vj_cross_attn_fwd` for the query-token attention); training the probe is the evals' job and stays with the reference
 (`forward` raises if a gradient is requested).  There is no CPU fallback.
 """

@@ -6,11 +6,11 @@ state dict with the reference's own keys.  Runs in float32 or float64.  Gradient
 autograd over these primitive ops.
 
 Pinning: the reference has no tests or golden vectors of its own (SURVEY.md section 4), so this file
-is pinned against the reference ITSELF: tests/golden/make_golden.py imports /root/reference, runs its
+is pinned against the reference ITSELF: tests/golden/make_golden.py imports a reference checkout, runs its
 unmodified modules on seeded inputs and commits the outputs to tests/golden/*.json|*.pt;
 tests/test_oracle_cpu.py checks every function below against those fixtures.
 
-Each function cites the reference lines it restates (paths relative to /root/reference).
+Each function cites the reference lines it restates (paths relative to the reference repository root).
 """
 import math
 

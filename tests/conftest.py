@@ -10,7 +10,7 @@ for p in (ROOT, os.path.join(ROOT, "tests", "golden")):
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA (B200) device; run with `-m gpu` under gpurun")
+    config.addinivalue_line("markers", "gpu: needs a CUDA (H100) device; run with `-m gpu`")
 
 
 @pytest.fixture(scope="session")

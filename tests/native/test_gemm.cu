@@ -1,4 +1,4 @@
-// Stand-alone bring-up / regression test for vj_gemm on a real B200 (no torch involved).
+// Stand-alone bring-up / regression test for vj_gemm on a real H100 (no torch involved).
 // Compares against a double-precision CPU reference on sampled rows and prints PASS/FAIL lines.
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>

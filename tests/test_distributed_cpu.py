@@ -1,4 +1,4 @@
-"""world_size-2 gloo tests of the multi-process host logic (runs on CPU; NCCL is exercised under gpurun):
+"""world_size-2 gloo tests of the multi-process host logic (runs on CPU; NCCL is exercised by the GPU tests):
 process-group bootstrap, the autograd-aware collectives, and the data-parallel gradient averaging contract
 (every rank ends a step with identical averaged gradients => identical replicas, no data-path collective
 other than the gradient all-reduce)."""

@@ -1,4 +1,4 @@
-"""2-GPU NCCL test of the data-parallel path (skipped on a 1-GPU box; `gpurun --gpus 2 -- pytest tests/test_gpu_multi.py -m gpu`):
+"""2-GPU NCCL test of the data-parallel path (skipped on a 1-GPU box; `pytest tests/test_gpu_multi.py -m gpu` on a 2-GPU one):
 the flat-buffer gradient exchange run inside the backward pass must leave on every rank the mean of the per-rank gradients
 of the same step computed without any exchange."""
 import copy

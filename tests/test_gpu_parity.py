@@ -684,7 +684,7 @@ def test_flat_grad_statistics_scaler_clip_and_loggers(dev):
 
 
 def test_attentive_probe_vs_reference_fixture(dev):
-    """SURVEY 8 f4: jepa_b200.pooler.AttentiveClassifier (vj_cross_attn_fwd + LayerNorm + tcgen05 GEMMs) vs the outputs the
+    """SURVEY 8 f4: jepa_b200.pooler.AttentiveClassifier (vj_cross_attn_fwd + LayerNorm + wgmma GEMMs) vs the outputs the
     UNMODIFIED reference modules produced for the same seeded weights and inputs (tests/golden/make_golden_pooler.py);
     head dims 64 / 32 / 80 / 128, complete_block on and off, class counts that are not multiples of 64."""
     from test_oracle_cpu import _build_probe, _pooler_fixture

@@ -1,77 +1,65 @@
-"""GPU parity against the REFERENCE ITSELF (-m gpu): the unmodified facebookresearch/jepa modules from baseline/_ref
-(tools/install_reference.sh) run on the same B200 in a subprocess - once under bf16 autocast (what app/vjepa/train.py:453
-does) and once in fp32 - on the seeded weights / clips / masks of tests/parity_util.py; our CUDA path runs the same step.
+"""GPU parity against the REFERENCE ITSELF (-m gpu): the unmodified facebookresearch/jepa modules ran the same step on
+an H100 (tools/ref_gpu.py `step`) - once under bf16 autocast (what app/vjepa/train.py:453 does) and once in fp32 - on the
+seeded weights / clips / masks of tests/parity_util.py; tests/golden/golden_reference_step.pt keeps both losses, the
+reference's own bf16-vs-fp32 rel-L2 of every tensor and a fixed seeded sample of every tensor of both runs
+(tests/golden/make_golden_reference.py).  Our CUDA path runs the same step and is compared on those samples.
 
 SURVEY 8c tolerances:
   (i)   ours-bf16 vs reference-bf16-autocast: rel-L2 <= 2e-2 on target / context / predictor outputs, loss |d| <= 2e-3;
         gradients rel-L2 <= 3e-2 (two bf16 computations with different rounding points)
   (iii) both against the reference in fp32 on the GPU: our error must be <= 2x the reference's own bf16 error (+ 2e-3)
-The product tree never imports baseline/_ref; nothing here reads /root/reference.
 """
-import json
 import os
-import subprocess
-import sys
 
 import pytest
 import torch
 
 from common import C1
+from make_golden_reference import flat_tensors, sample_index
 from parity_util import VITL_2B, rel_l2, run_c1_step_cuda
 
 pytestmark = pytest.mark.gpu
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF = os.path.join(ROOT, "baseline", "_ref")
 
 
 @pytest.fixture(scope="module")
 def dev():
     assert torch.cuda.is_available()
-    if not os.path.isdir(os.path.join(REF, "src")):
-        pytest.skip("baseline/_ref not installed (tools/install_reference.sh needs /root/reference; the install travels "
-                    "with the gpurun snapshot)")
     return torch.device("cuda:0")
 
 
-def _reference_step(cfg, tmp_path):
-    out = str(tmp_path / "ref_step.pt")
-    cmd = [sys.executable, os.path.join(ROOT, "tools", "ref_gpu.py"), "step", "--embed-dim", str(cfg["embed_dim"]),
-           "--heads", str(cfg["heads"]), "--depth", str(cfg["depth"]), "--pred-depth", str(cfg["pred_depth"]),
-           "--frames", str(cfg["num_frames"]), "--crop", str(cfg["crop_size"]), "--batch", str(cfg["batch"]),
-           "--mask-batch", str(cfg.get("mask_batch", cfg["batch"])), "--out", out]
-    env = {k: v for k, v in os.environ.items() if k != "PYTHONPATH"}
-    r = subprocess.run(cmd, capture_output=True, text=True, timeout=900, cwd="/tmp", env=env)
-    assert r.returncode == 0, r.stdout[-2000:] + r.stderr[-3000:]
-    info = json.loads(r.stdout.strip().splitlines()[-1])
-    assert "unavailable" not in info, info
-    return torch.load(out)
+@pytest.fixture(scope="module")
+def golden(golden_dir):
+    return torch.load(os.path.join(golden_dir, "golden_reference_step.pt"))
 
 
 @pytest.mark.parametrize("cfg", [C1, VITL_2B], ids=["c1_vit_tiny_12+12", "vitl16_2+2_blocks"])
-def test_step_vs_reference_on_same_gpu(dev, cfg, tmp_path):
-    ref = _reference_step(cfg, tmp_path)
+def test_step_vs_reference_on_same_gpu(dev, golden, cfg, request):
+    ref = golden[request.node.callspec.id]
     got = run_c1_step_cuda(dev, cfg=cfg)
-    rb, rf = ref["bf16"], ref["fp32"]
     report = {}
-    assert abs(got["loss_jepa"] - rb["loss_jepa"]) <= 2e-3, (got["loss_jepa"], rb["loss_jepa"])
-    assert abs(got["loss_jepa"] - rf["loss_jepa"]) <= 2e-3, (got["loss_jepa"], rf["loss_jepa"])
-    for key in ("h", "z_enc", "z"):
-        for i, a in enumerate(got[key]):
-            e_ours_b, e_ours_f = rel_l2(a, rb[key][i]), rel_l2(a, rf[key][i])
-            e_ref = rel_l2(rb[key][i], rf[key][i])
-            report[f"{key}[{i}]"] = (e_ours_b, e_ours_f, e_ref)
-            assert e_ours_b <= 2e-2, (key, i, e_ours_b)
-            assert e_ours_f <= 2 * e_ref + 2e-3, (key, i, e_ours_f, e_ref)
-    for key in ("enc_grad", "pred_grad"):
-        assert set(got[key]) == set(rf[key]), set(got[key]) ^ set(rf[key])
-        for n, a in got[key].items():
-            e_ours_b, e_ours_f = rel_l2(a, rb[key][n]), rel_l2(a, rf[key][n])
-            e_ref = rel_l2(rb[key][n], rf[key][n])
-            report[f"{key}.{n}"] = (e_ours_b, e_ours_f, e_ref)
-            assert e_ours_f <= max(3e-2, 2 * e_ref + 2e-3), (n, e_ours_f, e_ref)
-            assert e_ours_b <= max(3e-2, 3 * e_ref), (n, e_ours_b, e_ref)
+    assert abs(got["loss_jepa"] - ref["loss_bf16"]) <= 2e-3, (got["loss_jepa"], ref["loss_bf16"])
+    assert abs(got["loss_jepa"] - ref["loss_fp32"]) <= 2e-3, (got["loss_jepa"], ref["loss_fp32"])
+    ours = flat_tensors(got)
+    assert set(ours) == set(ref["keys"]), set(ours) ^ set(ref["keys"])
+    off = 0
+    for key, numel, e_ref in zip(ref["keys"], ref["numel"], ref["e_ref"].tolist()):
+        a = ours[key]
+        assert a.numel() == numel, key
+        idx = sample_index(numel, key)
+        s = a.reshape(-1)[idx].float()
+        rb, rf = ref["bf16"][off:off + idx.numel()].float(), ref["fp32"][off:off + idx.numel()]
+        off += idx.numel()
+        e_ours_b, e_ours_f = rel_l2(s, rb), rel_l2(s, rf)
+        report[key] = (e_ours_b, e_ours_f, e_ref)
+        if key.startswith(("enc_grad.", "pred_grad.")):
+            assert e_ours_f <= max(3e-2, 2 * e_ref + 2e-3), (key, e_ours_f, e_ref)
+            assert e_ours_b <= max(3e-2, 3 * e_ref), (key, e_ours_b, e_ref)
+        else:
+            assert e_ours_b <= 2e-2, (key, e_ours_b)
+            assert e_ours_f <= 2 * e_ref + 2e-3, (key, e_ours_f, e_ref)
+    assert off == ref["fp32"].numel()
     worst = sorted(report.items(), key=lambda kv: -kv[1][1])[:6]
-    print("ours-vs-ref-bf16 / ours-vs-ref-fp32 / ref-bf16-vs-ref-fp32 (rel-L2), worst by ours-vs-fp32:")
+    print("ours-vs-ref-bf16 / ours-vs-ref-fp32 (sampled) / ref-bf16-vs-ref-fp32 (full) rel-L2, worst by ours-vs-fp32:")
     for k, v in worst:
         print(f"  {k}: {v[0]:.4f} / {v[1]:.4f} / {v[2]:.4f}")
-    print("reference autocast dtypes:", rb["h_dtype"], rb["z_enc_dtype"], rb["z_dtype"])
+    print("reference autocast dtypes:", *ref["dtypes"])

@@ -2,7 +2,7 @@
 `python -m app.main` would call it (reference app/main.py:28-60, app/scaffold.py:16-21), on the synthetic dataset:
 CSV columns (train.py:199-209), reference-format checkpoint (train.py:307-324), resume through load_checkpoint
 (app/vjepa/utils.py:28-83) with the flat AdamW state re-aliased, and the saved encoder / predictor loading with
-strict=True into the UNMODIFIED reference modules when baseline/_ref is present."""
+strict=True into the UNMODIFIED reference modules when oracle/_ref is present."""
 import csv
 import json
 import os
@@ -82,7 +82,7 @@ def test_app_main_train_save_resume(tmp_path):
     assert not torch.equal(ck["encoder"][k], ck2["encoder"][k]) and not torch.equal(ck["target_encoder"][k], ck2["target_encoder"][k])
 
     # ---- the checkpoint is the reference's format: its own modules take it with strict=True
-    ref = os.path.join(ROOT, "baseline", "_ref")
+    ref = os.path.join(ROOT, "oracle", "_ref")
     if os.path.isdir(os.path.join(ref, "src")):
         code = f"""
 import sys, json

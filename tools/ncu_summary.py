@@ -59,7 +59,7 @@ def main():
     for r in sorted(data, key=lambda r: -int(r[isamp] or 0))[:12]:
         print(f"    {int(r[isamp] or 0):6d} ({100 * int(r[isamp] or 0) / max(tot, 1):4.1f}%)  {r[isrc][:90]}")
     proof = {k: v for k, v in mnem.items() if k.split(".")[0] in ("UTCHMMA", "UTCQMMA", "UTMALDG", "UTMASTG", "UTMAREDG", "LDTM", "STTM", "UTCBAR", "SYNCS", "MUFU", "FFMA2", "FMUL2", "FADD2", "HMUL2")}
-    print("  executed warp-instructions of the Blackwell-specific kinds:", ", ".join(f"{k}={v}" for k, v in sorted(proof.items())))
+    print("  executed warp-instructions of the architecture-specific kinds:", ", ".join(f"{k}={v}" for k, v in sorted(proof.items())))
 
 
 if __name__ == "__main__":

@@ -1,15 +1,16 @@
 #!/usr/bin/env python
-"""Run the UNMODIFIED reference (facebookresearch/jepa, installed into baseline/_ref by
-tools/install_reference.sh) on cuda:0.  Measurement / test infrastructure only - the product never imports this.
+"""Run the UNMODIFIED reference (facebookresearch/jepa, copied into oracle/_ref by
+oracle/make_ref.sh) on cuda:0.  Measurement / test infrastructure only - the product never imports this.
 
   bench : the reference's own training entry app.vjepa.train.main(args) at a BASELINE config (bf16 autocast, eager
           PyTorch: cuBLASLt GEMMs, SDPA, cuDNN Conv3d, c10d DDP over a 1-rank NCCL group), synthetic clips, its own
           MaskCollator (seed 0, first call reused like bench.py), timed by its own gpu_timer -> the CSV column
           `gpu-time(ms)` (src/utils/logging.py:14-31, app/vjepa/train.py:499).  This is the GPU bar SURVEY 8d asks
-          for: "the same reference code on the same B200".  --loggers off stubs grad_logger / adamw_logger
+          for: "the same reference code on the same GPU".  --loggers off stubs grad_logger / adamw_logger
           (the ~1000 host syncs per step, SURVEY 8d (A)); --loggers on is the as-shipped step (B).
   step  : one forward/backward of the reference modules on seeded weights / clips / masks (tests/golden/common.py)
-          at a chosen width/depth, in bf16 autocast AND in fp32, dumped to a .pt file for tests/test_gpu_reference.py.
+          at a chosen width/depth, in bf16 autocast AND in fp32, dumped to a .pt file (sampled into the golden fixture of
+          tests/test_gpu_reference.py by tests/golden/make_golden_reference.py).
 
 The repo root holds drop-in `src/` and `app/` packages with the reference's names, so this script must run in its own
 process with the repo root OFF sys.path.
@@ -24,10 +25,10 @@ import time
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
-REF = os.path.join(ROOT, "baseline", "_ref")
+REF = os.path.join(ROOT, "oracle", "_ref")
 sys.path = [p for p in sys.path if os.path.abspath(p or os.getcwd()) != ROOT]
 if not os.path.isdir(os.path.join(REF, "app")):
-    print(json.dumps({"impl": "reference-gpu", "unavailable": "baseline/_ref missing: run tools/install_reference.sh"}))
+    print(json.dumps({"impl": "reference-gpu", "unavailable": "oracle/_ref missing: run oracle/make_ref.sh"}))
     sys.exit(0)
 sys.path.insert(0, REF)
 sys.path.insert(1, os.path.join(ROOT, "tests", "golden"))

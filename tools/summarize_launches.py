@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Summarise an `ncu --metrics gpu__time_duration.sum --csv` launch list by kernel family.
 
-usage: python tools/summarize_launches.py gpurun_out/launches.csv [--skip N] [--steps K]
+usage: python tools/summarize_launches.py launches.csv [--skip N] [--steps K]
 Times under ncu are cold-cache and serialised: use the SHARES, never the absolute numbers, as bench values."""
 import csv
 import re
