@@ -5,10 +5,16 @@
 //   dQ = scale dS K, dK = scale dS^T Q.
 // Three kernels:
 //   attn_delta_kernel  : delta[h,t] = sum_d dO[t,h,d] O[t,h,d]                      (HBM-bound)
-//   attn_bwd_dkv_kernel: one CTA per 128-key tile (two warpgroups of 64 keys), loops over 64-query tiles; computes
-//                        S^T = K Q^T and dP^T = V dO^T directly in the transposed orientation so P^T / dS^T are register
-//                        A operands of dV += P^T dO and dK += dS^T Q, both accumulated in registers across the loop.
+//   attn_bwd_dkv_kernel: one CTA per 128-key tile (two consumer warpgroups of 64 keys), loops over 64-query tiles;
+//                        computes S^T = K Q^T and dP^T = V dO^T directly in the transposed orientation so P^T / dS^T are
+//                        register A operands of dV += P^T dO and dK += dS^T Q, both accumulated in registers across the loop.
 //   attn_bwd_dq_kernel : one CTA per 128-query tile, loops over 64-key tiles; dQ += dS K in registers.
+// Both loop kernels are warp-specialised like the forward: warpgroup 0 is the producer (one warp: TMA of the streamed
+// tiles into a 3-stage ring with full / empty mbarriers; for dK/dV it also stages the streamed queries' lse2 / delta in
+// shared memory, so the exps never wait on global loads), warpgroups 1-2 are the consumers, 64 resident rows each.
+// Without a CTA-wide barrier per tile the two consumers drift apart, so one's P / dS elementwise work runs under the
+// other's MMAs.  (Explicit ping-pong through named barriers, and issuing the next S / dP ahead of the current gradient
+// MMAs, were both measured slower on these short-K tiles.)  The arithmetic per resident row is unchanged by the schedule.
 // P is recomputed from the forward's log2-domain LSE.  Same qkv / O layouts as attn_fwd.cu; the
 // gradient dqkv has the qkv layout [T, 3*H*HD] so the qkv wgrad/dgrad GEMMs consume it directly.
 #include <stdlib.h>
@@ -18,8 +24,9 @@
 
 namespace vj {
 
-constexpr int kBwdThreads = 256;
+constexpr int kBwdThreads = 384;
 constexpr int kBwdStream = 64;   // rows of the streamed (query or key) tiles
+constexpr int kBwdStages = 3;
 
 struct AttnBwdParams {
   const int* cu_seqlens;
@@ -33,13 +40,17 @@ struct AttnBwdParams {
 template <int HD>
 struct BwdCfg {
   using A = AttnCfg<HD>;
-  // two resident [128 x HD] tiles (T0, T1) and two stages of the two streamed [64 x HD] tiles
+  // two resident [128 x HD] tiles (T0, T1), kBwdStages stages of the two streamed [64 x HD] tiles and of the streamed
+  // rows' lse2 / delta (dK/dV kernel only)
   static constexpr int RES = A::template tile_bytes<128>();
   static constexpr int STR = A::template tile_bytes<kBwdStream>();
   static constexpr int T0 = 0, T1 = RES;
   static constexpr int S_OFF = 2 * RES;                 // stage st: tile a at S_OFF + st * 2 * STR, tile b at + STR
-  static constexpr int BAR_OFF = S_OFF + 4 * STR;
-  static constexpr int SMEM_BYTES = BAR_OFF + 64 + 1024;
+  static constexpr int STAT_OFF = S_OFF + kBwdStages * 2 * STR;   // stage st: lse2 at + st * STAT, delta at + STAT / 2
+  static constexpr int STAT = 2 * kBwdStream * 4;
+  static constexpr int BAR_OFF = STAT_OFF + kBwdStages * STAT;    // resident, full[stages], empty[stages]
+  static constexpr int SMEM_BYTES = BAR_OFF + 8 * (1 + 2 * kBwdStages) + 1024;
+  static_assert(SMEM_BYTES <= 232448, "attention backward shared memory budget exceeded");
 };
 
 // ---------------------------------------------------------------------------------------------
@@ -94,46 +105,75 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmRes, const __grid_constant
 
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + B::BAR_OFF);
   const uint32_t bar_res = smem_u32(bars + 0);
-  const uint32_t bar_s0 = smem_u32(bars + 1);   // 2 stages
+  const uint32_t full0 = smem_u32(bars + 1);                 // stage st: + 8 st
+  const uint32_t empty0 = smem_u32(bars + 1 + kBwdStages);
   const uint32_t sT0 = smem_u32(smem + B::T0), sT1 = smem_u32(smem + B::T1), sS = smem_u32(smem + B::S_OFF);
+  const uint32_t sStat = smem_u32(smem + B::STAT_OFF);
+  const float* lse_h = p.lse2 + (long long)head * p.T + row_begin;
+  const float* del_h = p.delta + (long long)head * p.T + row_begin;
+  const int wg = threadIdx.x >> 7;
+  const int lane = threadIdx.x & 31;
 
-  // resident: DKV -> T0 = K, T1 = V;  dQ -> T0 = Q, T1 = dO.   streamed: DKV -> a = Q_i, b = dO_i;  dQ -> a = K_j, b = V_j
-  auto load_stream = [&](int i) {   // thread 0 only
-    const int st = i & 1;
-    const uint32_t a = sS + st * 2 * B::STR, b = a + B::STR, bar = bar_s0 + 8 * st;
-    const int r0 = row_begin + i * kBwdStream;
-    mbar_expect_tx(bar, 2 * B::STR);
-    if (DKV) {
-      attn_load_tile<HD, kBwdStream>(a, &tmStr, bar, head * HD, r0);
-      attn_load_tile<HD, kBwdStream>(b, &tmDO, bar, head * HD, r0);
-    } else {
-      attn_load_tile<HD, kBwdStream>(a, &tmStr, bar, HHD + head * HD, r0);
-      attn_load_tile<HD, kBwdStream>(b, &tmStr, bar, 2 * HHD + head * HD, r0);
-    }
-  };
   if (threadIdx.x == 0) {
     mbar_init(bar_res, 1);
-    mbar_init(bar_s0, 1);
-    mbar_init(bar_s0 + 8, 1);
-    fence_mbar_init();
-    mbar_expect_tx(bar_res, 2 * B::RES);
-    if (DKV) {
-      attn_load_tile<HD, 128>(sT0, &tmRes, bar_res, HHD + head * HD, row_begin + t0);
-      attn_load_tile<HD, 128>(sT1, &tmRes, bar_res, 2 * HHD + head * HD, row_begin + t0);
-    } else {
-      attn_load_tile<HD, 128>(sT0, &tmRes, bar_res, head * HD, row_begin + t0);
-      attn_load_tile<HD, 128>(sT1, &tmDO, bar_res, head * HD, row_begin + t0);
+    for (int st = 0; st < kBwdStages; ++st) {
+      mbar_init(full0 + 8 * st, DKV ? 32 : 1);   // dK/dV: every producer lane arrives after its lse2 / delta stores
+      mbar_init(empty0 + 8 * st, 8);             // one arrive per consumer warp
     }
-    load_stream(0);
-    if (n_it > 1) load_stream(1);
+    fence_mbar_init();
   }
   __syncthreads();
 
-  const int wg = threadIdx.x >> 7;
-  const int lane = threadIdx.x & 31;
-  const int r = wg * 64 + ((threadIdx.x >> 5) & 3) * 16 + (lane >> 2);   // first fragment row in the resident tile
-  const float* lse_h = p.lse2 + (long long)head * p.T + row_begin;
-  const float* del_h = p.delta + (long long)head * p.T + row_begin;
+  // resident: DKV -> T0 = K, T1 = V;  dQ -> T0 = Q, T1 = dO.   streamed: DKV -> a = Q_i, b = dO_i;  dQ -> a = K_j, b = V_j
+  if (wg == 0) {
+    // ------------------------------------------------------------------ producer (warp 0)
+    setmaxnreg_dec<40>();
+    if (threadIdx.x < 32) {
+      if (lane == 0) {
+        mbar_expect_tx(bar_res, 2 * B::RES);
+        if (DKV) {
+          attn_load_tile<HD, 128>(sT0, &tmRes, bar_res, HHD + head * HD, row_begin + t0);
+          attn_load_tile<HD, 128>(sT1, &tmRes, bar_res, 2 * HHD + head * HD, row_begin + t0);
+        } else {
+          attn_load_tile<HD, 128>(sT0, &tmRes, bar_res, head * HD, row_begin + t0);
+          attn_load_tile<HD, 128>(sT1, &tmDO, bar_res, head * HD, row_begin + t0);
+        }
+      }
+      for (int i = 0; i < n_it; ++i) {
+        const int st = i % kBwdStages;
+        const uint32_t a = sS + st * 2 * B::STR, b = a + B::STR, bar = full0 + 8 * st;
+        const int c0 = i * kBwdStream;
+        mbar_wait(empty0 + 8 * st, ((i / kBwdStages) & 1) ^ 1);
+        if (DKV) {
+#pragma unroll
+          for (int k = 0; k < kBwdStream / 32; ++k) {
+            const int col = c0 + 32 * k + lane;
+            const uint32_t dst = sStat + st * B::STAT + (32 * k + lane) * 4;
+            sts32f(dst, col < len ? lse_h[col] : 0.f);
+            sts32f(dst + B::STAT / 2, col < len ? del_h[col] : 0.f);
+          }
+        }
+        if (lane == 0) {
+          mbar_expect_tx(bar, 2 * B::STR);
+          if (DKV) {
+            attn_load_tile<HD, kBwdStream>(a, &tmStr, bar, head * HD, row_begin + c0);
+            attn_load_tile<HD, kBwdStream>(b, &tmDO, bar, head * HD, row_begin + c0);
+          } else {
+            attn_load_tile<HD, kBwdStream>(a, &tmStr, bar, HHD + head * HD, row_begin + c0);
+            attn_load_tile<HD, kBwdStream>(b, &tmStr, bar, 2 * HHD + head * HD, row_begin + c0);
+          }
+        } else if (DKV) {
+          mbar_arrive(bar);
+        }
+      }
+    }
+    return;
+  }
+
+  // -------------------------------------------------------------------- consumers
+  setmaxnreg_inc<232>();
+  const int cw = wg - 1;   // which 64-row half of the resident tile
+  const int r = cw * 64 + ((threadIdx.x >> 5) & 3) * 16 + (lane >> 2);   // first fragment row in the resident tile
   float acc0[HD / 2], acc1[HD / 2];   // DKV: dV, dK;  dQ: dQ (acc1 unused)
 #pragma unroll
   for (int i = 0; i < HD / 2; ++i) { acc0[i] = 0.f; acc1[i] = 0.f; }
@@ -146,23 +186,22 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmRes, const __grid_constant
       row_del[h] = q < len ? del_h[q] : 0.f;
     }
   }
-
   mbar_wait(bar_res, 0);
   for (int i = 0; i < n_it; ++i) {
-    const int st = i & 1;
+    const int st = i % kBwdStages;
     const uint32_t sa = sS + st * 2 * B::STR, sb = sa + B::STR;
     const int c0 = i * kBwdStream;   // first streamed row (relative to the sequence)
-    mbar_wait(bar_s0 + 8 * st, (i >> 1) & 1);
+    mbar_wait(full0 + 8 * st, (i / kBwdStages) & 1);
     // DKV: x = S^T = K Q_i^T, y = dP^T = V dO_i^T;   dQ: x = S = Q K_j^T, y = dP = dO V_j^T
     float x[kBwdStream / 2], y[kBwdStream / 2];
     wgmma_fence();
 #pragma unroll
     for (int kk = 0; kk < HD / 16; ++kk)
-      wgmma_ss<kBwdStream, 0, 0>(x, attn_kmajor_desc<HD, 128>(sT0, wg * 64, kk), attn_kmajor_desc<HD, kBwdStream>(sa, 0, kk),
+      wgmma_ss<kBwdStream, 0, 0>(x, attn_kmajor_desc<HD, 128>(sT0, cw * 64, kk), attn_kmajor_desc<HD, kBwdStream>(sa, 0, kk),
                                  kk > 0);
 #pragma unroll
     for (int kk = 0; kk < HD / 16; ++kk)
-      wgmma_ss<kBwdStream, 0, 0>(y, attn_kmajor_desc<HD, 128>(sT1, wg * 64, kk), attn_kmajor_desc<HD, kBwdStream>(sb, 0, kk),
+      wgmma_ss<kBwdStream, 0, 0>(y, attn_kmajor_desc<HD, 128>(sT1, cw * 64, kk), attn_kmajor_desc<HD, kBwdStream>(sb, 0, kk),
                                  kk > 0);
     wgmma_commit();
     wgmma_wait<0>();
@@ -174,10 +213,13 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmRes, const __grid_constant
     for (int c = 0; c < kBwdStream / 8; ++c)
 #pragma unroll
       for (int e = 0; e < 2; ++e) {
-        const int col = c0 + 8 * c + 2 * (lane & 3) + e;
-        const bool col_ok = col < len;
+        const int col = 8 * c + 2 * (lane & 3) + e;   // in the streamed tile
+        const bool col_ok = c0 + col < len;
         float cl = 0.f, cd = 0.f;
-        if (DKV && col_ok) { cl = lse_h[col]; cd = del_h[col]; }
+        if (DKV) {
+          cl = lds32f(sStat + st * B::STAT + col * 4);
+          cd = lds32f(sStat + st * B::STAT + B::STAT / 2 + col * 4);
+        }
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
           const float l2 = DKV ? cl : row_lse[h], dl = DKV ? cd : row_del[h];
@@ -209,8 +251,8 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmRes, const __grid_constant
     wgmma_wait<0>();
     wgmma_fence_regs(acc0);
     wgmma_fence_regs(acc1);
-    __syncthreads();   // both warpgroups are done with stage st
-    if (threadIdx.x == 0 && i + 2 < n_it) load_stream(i + 2);
+    __syncwarp();
+    if (lane == 0) mbar_arrive(empty0 + 8 * st);   // this warp is done with stage st
   }
 
   __nv_bfloat16* rows = p.dqkv + (long long)(row_begin + t0) * 3 * HHD + head * HD;

@@ -8,10 +8,21 @@
 // layout the qkv GEMM epilogue writes), O bf16 [T, H*HD], lse2 fp32 [H, T] (log2 domain:
 // m*scale*log2e + log2(l)).  Sequences are row ranges [cu[s], cu[s+1]).
 //
-// One CTA = one 128-row query tile of one (sequence, head), two warpgroups of 64 query rows each.  K_j / V_j tiles of
-// 128 keys stream through a two-stage TMA ring (thread 0 refills a stage as soon as both warpgroups are done with it).
-// Per tile: S = Q K_j^T (wgmma, both operands in smem), online softmax on the accumulator fragment in registers,
-// O += P V_j with P as the register A operand (no shared-memory round trip) and V_j read MN-major.
+// One CTA = one 128-row query tile of one (sequence, head); K_j / V_j tiles of 128 keys stream through a 3-stage TMA ring.
+// Warp-specialised, three warpgroups (the FlashAttention-3 schedule):
+//   warpgroup 0   : TMA producer (one thread loads Q, then K_j / V_j into stage j % 3 once both consumers released it;
+//                   per-stage full (tx-count) and empty (one arrive per consumer warp) mbarriers)
+//   warpgroups 1-2: consumers, 64 query rows each.  S = Q K_j^T (wgmma, both operands in smem), online softmax on the
+//                   accumulator fragment in registers, O += P V_j with P as the register A operand (no shared-memory round
+//                   trip) and V_j read MN-major.
+// Two overlaps keep the tensor cores busy while the exps run:
+//   - inside a warpgroup, S_j = Q K_j^T is issued together with O += P_{j-1} V_{j-1} (P_{j-1} held as bf16 fragments), so
+//     the softmax of S_j runs under P_{j-1} V_{j-1}; O is rescaled by alpha_j once that MMA has retired;
+//   - between the warpgroups, two named barriers make them take turns issuing (ping-pong), so one warpgroup's softmax runs
+//     under the other's MMAs.
+// Only the ragged last KV tile of a sequence pays for the key mask.
+// The per-row arithmetic and its order over the KV tiles are those of a plain one-tile-at-a-time loop, so O and lse2 do
+// not depend on the schedule.
 #include <stdlib.h>
 
 #include "attn_common.cuh"
@@ -19,8 +30,9 @@
 
 namespace vj {
 
-constexpr int kFwdThreads = 256;
+constexpr int kFwdThreads = 384;
 constexpr int kFwdKV = 128;   // keys per tile
+constexpr int kFwdStages = 3;
 
 struct AttnFwdParams {
   const int* cu_seqlens;
@@ -36,11 +48,16 @@ struct FwdCfg {
   using A = AttnCfg<HD>;
   static constexpr int TILE = A::template tile_bytes<128>();
   static constexpr int Q_OFF = 0;
-  static constexpr int K_OFF = TILE;          // 2 stages
-  static constexpr int V_OFF = 3 * TILE;      // 2 stages
-  static constexpr int BAR_OFF = 5 * TILE;
-  static constexpr int SMEM_BYTES = BAR_OFF + 64 + 1024;
+  static constexpr int K_OFF = TILE;                          // kFwdStages stages
+  static constexpr int V_OFF = K_OFF + kFwdStages * TILE;     // kFwdStages stages
+  static constexpr int BAR_OFF = V_OFF + kFwdStages * TILE;   // Q, full[stages], empty[stages]
+  static constexpr int SMEM_BYTES = BAR_OFF + 8 * (1 + 2 * kFwdStages) + 1024;
+  static_assert(SMEM_BYTES <= 232448, "attention forward shared memory budget exceeded");
 };
+
+// Ping-pong between the consumer warpgroups cw = 0, 1: named barrier 1 + cw opens cw's turn to issue MMAs.
+VJ_DEVINL void pingpong_wait_turn(int cw) { named_bar_sync(1 + cw, 256); }
+VJ_DEVINL void pingpong_pass_turn(int cw) { named_bar_arrive(2 - cw, 256); }
 
 template <int HD>
 __global__ void __launch_bounds__(kFwdThreads, 1)
@@ -58,66 +75,87 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQKV, const AttnFwdParams p
 
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + F::BAR_OFF);
   const uint32_t bar_q = smem_u32(bars + 0);
-  const uint32_t bar_kv0 = smem_u32(bars + 1);   // 2 stages: +0, +8
+  const uint32_t full0 = smem_u32(bars + 1);                 // stage st: + 8 st
+  const uint32_t empty0 = smem_u32(bars + 1 + kFwdStages);
   const uint32_t sQ = smem_u32(smem + F::Q_OFF), sK = smem_u32(smem + F::K_OFF), sV = smem_u32(smem + F::V_OFF);
   const int HHD = p.H * HD;
+  const int wg = threadIdx.x >> 7;
 
-  auto load_kv = [&](int j) {   // thread 0 only
-    const int st = j & 1;
-    mbar_expect_tx(bar_kv0 + 8 * st, 2 * F::TILE);
-    attn_load_tile<HD, 128>(sK + st * F::TILE, &tmQKV, bar_kv0 + 8 * st, HHD + head * HD, row_begin + j * kFwdKV);
-    attn_load_tile<HD, 128>(sV + st * F::TILE, &tmQKV, bar_kv0 + 8 * st, 2 * HHD + head * HD, row_begin + j * kFwdKV);
-  };
   if (threadIdx.x == 0) {
     mbar_init(bar_q, 1);
-    mbar_init(bar_kv0, 1);
-    mbar_init(bar_kv0 + 8, 1);
+    for (int st = 0; st < kFwdStages; ++st) {
+      mbar_init(full0 + 8 * st, 1);
+      mbar_init(empty0 + 8 * st, 8);   // one arrive per consumer warp
+    }
     fence_mbar_init();
     tma_prefetch_desc(&tmQKV);
-    mbar_expect_tx(bar_q, F::TILE);
-    attn_load_tile<HD, 128>(sQ, &tmQKV, bar_q, head * HD, row_begin + q0);
-    load_kv(0);
-    if (n_kv > 1) load_kv(1);
   }
   __syncthreads();
 
-  const int wg = threadIdx.x >> 7;
+  if (wg == 0) {
+    // ------------------------------------------------------------------ TMA producer
+    setmaxnreg_dec<40>();
+    if (threadIdx.x == 0) {
+      mbar_expect_tx(bar_q, F::TILE);
+      attn_load_tile<HD, 128>(sQ, &tmQKV, bar_q, head * HD, row_begin + q0);
+      for (int j = 0; j < n_kv; ++j) {
+        const int st = j % kFwdStages;
+        mbar_wait(empty0 + 8 * st, ((j / kFwdStages) & 1) ^ 1);
+        const uint32_t fb = full0 + 8 * st;
+        mbar_expect_tx(fb, 2 * F::TILE);
+        attn_load_tile<HD, 128>(sK + st * F::TILE, &tmQKV, fb, HHD + head * HD, row_begin + j * kFwdKV);
+        attn_load_tile<HD, 128>(sV + st * F::TILE, &tmQKV, fb, 2 * HHD + head * HD, row_begin + j * kFwdKV);
+      }
+    }
+    return;
+  }
+
+  // -------------------------------------------------------------------- consumers
+  setmaxnreg_inc<232>();
+  const int cw = wg - 1;   // which 64-row half of the query tile
   const int lane = threadIdx.x & 31;
-  const int r = wg * 64 + ((threadIdx.x >> 5) & 3) * 16 + (lane >> 2);   // this thread's first row in the tile (+8: second)
+  const int r = cw * 64 + ((threadIdx.x >> 5) & 3) * 16 + (lane >> 2);   // this thread's first row in the tile (+8: second)
   float o[HD / 2];
 #pragma unroll
   for (int i = 0; i < HD / 2; ++i) o[i] = 0.f;
   float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
+  float s[kFwdKV / 2];              // S_j, then P_j (fp32)
+  uint32_t pf[kFwdKV / 16][4];      // P_{j-1} as bf16 A fragments, read by the in-flight P_{j-1} V_{j-1}
+  if (cw == 1) pingpong_pass_turn(cw);   // warpgroup 0 issues first
 
-  mbar_wait(bar_q, 0);
-  for (int j = 0; j < n_kv; ++j) {
-    const int st = j & 1;
-    const int valid = min(kFwdKV, len - j * kFwdKV);
-    mbar_wait(bar_kv0 + 8 * st, (j >> 1) & 1);
-    float s[kFwdKV / 2];
-    wgmma_fence();
+  auto issue_s = [&](int st) {
 #pragma unroll
     for (int kk = 0; kk < HD / 16; ++kk)
-      wgmma_ss<kFwdKV, 0, 0>(s, attn_kmajor_desc<HD, 128>(sQ, wg * 64, kk),
+      wgmma_ss<kFwdKV, 0, 0>(s, attn_kmajor_desc<HD, 128>(sQ, cw * 64, kk),
                              attn_kmajor_desc<HD, 128>(sK + st * F::TILE, 0, kk), kk > 0);
     wgmma_commit();
-    wgmma_wait<0>();
-    wgmma_fence_regs(s);
-
-    // ---- online softmax on the fragment: s[4c + 2h + e] = row r + 8h, key 8c + 2(lane % 4) + e
-    float alpha[2];
+  };
+  auto issue_pv = [&](int st) {
+#pragma unroll
+    for (int kk = 0; kk < kFwdKV / 16; ++kk) wgmma_rs<HD, 1>(o, pf[kk], attn_mnmajor_desc<HD, 128>(sV + st * F::TILE, kk), 1);
+    wgmma_commit();
+  };
+  auto release = [&](int st) {
+    __syncwarp();
+    if (lane == 0) mbar_arrive(empty0 + 8 * st);
+  };
+  // ---- online softmax of tile j on the fragment: s[4c + 2h + e] = row r + 8h, key 8c + 2(lane % 4) + e
+  auto softmax = [&](int j, float (&alpha)[2]) {
+    const int valid = len - j * kFwdKV;
+    if (valid < kFwdKV) {   // ragged last tile
+#pragma unroll
+      for (int c = 0; c < kFwdKV / 8; ++c)
+#pragma unroll
+        for (int e = 0; e < 4; ++e)
+          if (8 * c + 2 * (lane & 3) + (e & 1) >= valid) s[4 * c + e] = -INFINITY;
+    }
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       float mx = -INFINITY;
 #pragma unroll
       for (int c = 0; c < kFwdKV / 8; ++c)
 #pragma unroll
-        for (int e = 0; e < 2; ++e) {
-          const int key = 8 * c + 2 * (lane & 3) + e;
-          float& v = s[4 * c + 2 * h + e];
-          if (key >= valid) v = -INFINITY;
-          mx = fmaxf(mx, v);
-        }
+        for (int e = 0; e < 2; ++e) mx = fmaxf(mx, s[4 * c + 2 * h + e]);
       mx = quad_max(mx);
       const float m_new = fmaxf(m_run[h], mx);
       alpha[h] = ex2_approx((m_run[h] - m_new) * p.scale_log2);   // 0 on the first tile (m_run = -inf)
@@ -134,27 +172,62 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQKV, const AttnFwdParams p
         }
       l_run[h] = l_run[h] * alpha[h] + sum;   // per-thread partial; the quad is summed once at the end
     }
+  };
+  auto rescale_o = [&](const float (&alpha)[2]) {
 #pragma unroll
     for (int c = 0; c < HD / 8; ++c) {
       o[4 * c + 0] *= alpha[0]; o[4 * c + 1] *= alpha[0];
       o[4 * c + 2] *= alpha[1]; o[4 * c + 3] *= alpha[1];
     }
+  };
+  auto pack_p = [&]() {
+#pragma unroll
+    for (int kk = 0; kk < kFwdKV / 16; ++kk) acc_to_afrag(s, kk, pf[kk]);
+  };
 
-    // ---- O += P V_j
+  mbar_wait(bar_q, 0);
+  // tile 0: S_0 alone
+  float alpha[2];
+  pingpong_wait_turn(cw);
+  mbar_wait(full0, 0);
+  wgmma_fence();
+  issue_s(0);
+  pingpong_pass_turn(cw);
+  wgmma_wait<0>();
+  wgmma_fence_regs(s);
+  softmax(0, alpha);
+  rescale_o(alpha);
+  pack_p();
+  // tile j: S_j together with P_{j-1} V_{j-1}
+  for (int j = 1; j < n_kv; ++j) {
+    const int st = j % kFwdStages, st_prev = (j - 1) % kFwdStages;
+    pingpong_wait_turn(cw);
+    mbar_wait(full0 + 8 * st, (j / kFwdStages) & 1);
     wgmma_fence_regs(o);
     wgmma_fence();
-#pragma unroll
-    for (int kk = 0; kk < kFwdKV / 16; ++kk) {
-      uint32_t a[4];
-      acc_to_afrag(s, kk, a);
-      wgmma_rs<HD, 1>(o, a, attn_mnmajor_desc<HD, 128>(sV + st * F::TILE, kk), 1);
-    }
-    wgmma_commit();
+    issue_s(st);
+    issue_pv(st_prev);
+    pingpong_pass_turn(cw);
+    wgmma_wait<1>();   // S_j is ready, P_{j-1} V_{j-1} may still run
+    wgmma_fence_regs(s);
+    softmax(j, alpha);
     wgmma_wait<0>();
     wgmma_fence_regs(o);
-    __syncthreads();   // both warpgroups are done with stage st
-    if (threadIdx.x == 0 && j + 2 < n_kv) load_kv(j + 2);
+    wgmma_fence_regs(pf);
+    release(st_prev);
+    rescale_o(alpha);
+    pack_p();
   }
+  // last P V
+  pingpong_wait_turn(cw);
+  wgmma_fence_regs(o);
+  wgmma_fence();
+  issue_pv((n_kv - 1) % kFwdStages);
+  pingpong_pass_turn(cw);
+  wgmma_wait<0>();
+  wgmma_fence_regs(o);
+  wgmma_fence_regs(pf);
+  if (cw == 0) pingpong_wait_turn(cw);   // takes warpgroup 1's last pass, so both barriers end balanced
 
   // ---- epilogue: O / l -> bf16, lse2 (log2 domain)
   float inv[2];

@@ -84,6 +84,20 @@ VJ_DEVINL void mbar_wait(uint32_t bar, uint32_t parity) {
   }
 }
 
+// Named hardware barriers (ids 1..15; 0 is __syncthreads).  `threads` counts every thread that syncs or arrives.
+VJ_DEVINL void named_bar_sync(int id, int threads) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory");
+}
+VJ_DEVINL void named_bar_arrive(int id, int threads) {
+  asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(threads) : "memory");
+}
+
+// Warp-specialised kernels: the TMA producer warpgroup gives registers back, the consumer warpgroups take them.
+template <int N>
+VJ_DEVINL void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N>
+VJ_DEVINL void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
+
 // ---------------------------------------------------------------------------------------
 // device: TMA
 // ---------------------------------------------------------------------------------------

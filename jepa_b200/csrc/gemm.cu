@@ -124,9 +124,6 @@ VJ_DEVINL float gelu_grad_fast(float x) {
   return d;
 }
 
-VJ_DEVINL void setmaxnreg_dec40() { asm volatile("setmaxnreg.dec.sync.aligned.u32 40;"); }
-VJ_DEVINL void setmaxnreg_inc232() { asm volatile("setmaxnreg.inc.sync.aligned.u32 232;"); }
-
 // EPI is a compile-time epilogue kind so that e.g. the plain / GELU kernels carry none of the aux code.
 template <int BN, bool A_MN, bool B_MN, bool OUT_F32, int EPI, bool AUX32>
 __global__ void __launch_bounds__(kGemmThreads, 1)
@@ -154,7 +151,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
 
   if (wg == 0) {
     // ------------------------------------------------------------------ TMA producer
-    setmaxnreg_dec40();
+    setmaxnreg_dec<40>();
     if (threadIdx.x == 0) {
       int stage = 0;
       uint32_t phase = 0;
@@ -193,7 +190,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
   }
 
   // -------------------------------------------------------------------- consumers
-  setmaxnreg_inc232();
+  setmaxnreg_inc<232>();
   const int cw = wg - 1;                    // which 64-row half of the tile
   const int warp_in_wg = (threadIdx.x >> 5) & 3;
   const int lane = threadIdx.x & 31;
