@@ -147,6 +147,19 @@ int vj_token_std_accum(const void* z, float* pstd, int B, int K, int D, float ep
  * (k | v halves, head-major).  HD in {32, 64, 80, 128}. */
 int vj_cross_attn_fwd(const void* q, const void* kv, void* out, int B, int nq, int S, int H, int HD, float scale,
                       void* stream);
+/* Same as vj_cross_attn_fwd (out bitwise identical), and also writes the softmax statistics lse2 fp32 [B*nq, H]
+ * (row b*nq + j, column head; log2 domain: lse2 = log2 sum_k exp2(scale log2e q.k)) for the backward. */
+int vj_cross_attn_fwd_lse(const void* q, const void* kv, void* out, float* lse2, int B, int nq, int S, int H, int HD,
+                          float scale, void* stream);
+/* Bytes of fp32 workspace vj_cross_attn_bwd needs (per-key-chunk dq partials). */
+size_t vj_cross_attn_bwd_workspace(int B, int nq, int S, int H, int HD);
+/* Backward of the above (autograd of modules.py:138-153 for training the attentive probe).  From q, kv, out, dout
+ * (bf16, layouts as in the forward) and lse2: dq fp32 [B*nq, H*HD], dkv bf16 [B*S, 2*H*HD] (dk | dv halves).
+ * dk / dv sum over the clip's nq queries.  Deterministic: no atomics, every dkv element is written once and dq is
+ * reduced over key chunks in a fixed order.  HD in {32, 64, 80, 128}. */
+int vj_cross_attn_bwd(const void* q, const void* kv, const void* out, const void* dout, const float* lse2, float* dq,
+                      void* dkv, void* workspace, size_t ws_bytes, int B, int nq, int S, int H, int HD, float scale,
+                      void* stream);
 
 /* ---- flat-buffer parameter kernels ------------------------------------------------------------ */
 /* dst bf16[n] = src fp32[n]: the per-step bf16 shadow of the fp32 master weights (what autocast's

@@ -39,6 +39,9 @@ SIGNATURES = {
     "vj_lp_loss_fwd": (I, [P, P, P, L, F, F, P]),
     "vj_lp_loss_bwd": (I, [P, P, P, F, P, L, F, P]),
     "vj_cross_attn_fwd": (I, [P, P, P, I, I, I, I, I, F, P]),
+    "vj_cross_attn_fwd_lse": (I, [P, P, P, P, I, I, I, I, I, F, P]),
+    "vj_cross_attn_bwd_workspace": (Z, [I, I, I, I, I]),
+    "vj_cross_attn_bwd": (I, [P, P, P, P, P, P, P, P, Z, I, I, I, I, I, F, P]),
     "vj_token_std_bwd": (I, [P, P, P, F, P, I, I, I, F, F, P]),
     "vj_cast_f32_bf16": (I, [P, P, L, P]),
     "vj_head_pad": (I, [P, I, P, I, L, I, I, I, L, I, P]),

@@ -215,6 +215,25 @@ def cross_attn_fwd(q, kv, out, B, nq, S, H, hd, scale):
     return out
 
 
+def cross_attn_fwd_lse(q, kv, out, lse2, B, nq, S, H, hd, scale):
+    """cross_attn_fwd that also writes the softmax statistics lse2 fp32 [B*nq, H] (log2 domain) for the backward."""
+    _chk(q, BF16, "q"); _chk(kv, BF16, "kv"); _chk(out, BF16, "out"); _chk(lse2, F32, "lse2")
+    _lib.call("vj_cross_attn_fwd_lse", _p(q), _p(kv), _p(out), _p(lse2), B, nq, S, H, hd, float(scale), _s())
+    return out
+
+
+def cross_attn_bwd(q, kv, out, dout, lse2, dq, dkv, B, nq, S, H, hd, scale):
+    """dq fp32 [B*nq, H*hd] and dkv bf16 [B*S, 2*H*hd] of cross_attn_fwd_lse."""
+    for t, n in ((q, "q"), (kv, "kv"), (out, "out"), (dout, "dout"), (dkv, "dkv")):
+        _chk(t, BF16, n)
+    _chk(lse2, F32, "lse2"); _chk(dq, F32, "dq")
+    need = _lib.load().vj_cross_attn_bwd_workspace(B, nq, S, H, hd)
+    ws = torch.empty(max(need, 4), dtype=torch.uint8, device=q.device)
+    _lib.call("vj_cross_attn_bwd", _p(q), _p(kv), _p(out), _p(dout), _p(lse2), _p(dq), _p(dkv), _p(ws), ws.numel(),
+              B, nq, S, H, hd, float(scale), _s())
+    return dq, dkv
+
+
 def token_std_accum(z, pstd, weight, eps=1e-4):
     _chk(z, BF16, "z"); _chk(pstd, F32, "pstd")
     B, K, D = z.shape

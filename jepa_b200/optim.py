@@ -9,7 +9,9 @@ tensors instead of syncing the host: the skip-on-overflow decision is taken insi
 Fast path: when all parameters of a backbone live in a FlatParamStore and their gradients are the slices
 of ONE flat gradient buffer (what our backward produces), the whole backbone is updated by a single
 `vj_adamw_flat` launch; a per-64-element group table carries each tensor's (lr, weight_decay) group.
-Anything else falls back to one `vj_adamw_step` launch per tensor.
+Anything else falls back to one `vj_adamw_step` launch per tensor.  A trainable member of a store whose `.grad` is None
+(the attentive probe's `proj`, which the reference never applies) is treated as torch.optim.AdamW treats it: it is not
+updated and gets no optimizer state.
 """
 import ctypes
 
@@ -58,11 +60,16 @@ class FlatAdamW(torch.optim.Optimizer):
                     by_store.setdefault(id(store), (store, []))[1].append((gi, p))
         return by_store, leftovers
 
+    @staticmethod
+    def _stepped(p):
+        """Members the flat step updates: trainable and with a gradient this step (torch.optim.AdamW skips the rest)."""
+        return p.requires_grad and p.grad is not None
+
     def _flat_state(self, store, members):
-        key = (store.flat.data_ptr(), store.total, tuple((gi, id(p)) for gi, p in members))
+        key = (store.flat.data_ptr(), store.total, tuple((gi, id(p), self._stepped(p)) for gi, p in members))
         st = self._flat.get(id(store))
         if st is not None and st["key"] == key:
-            p0 = next(p for _, p in members if p.requires_grad)   # frozen members carry no state
+            p0 = next(p for _, p in members if self._stepped(p))   # frozen / gradient-less members carry no state
             off0 = store.offsets[p0._vj_name][0]
             ea = self.state.get(p0, {}).get("exp_avg")
             if ea is not None and ea.data_ptr() == st["m"].data_ptr() + 4 * off0:
@@ -71,7 +78,7 @@ class FlatAdamW(torch.optim.Optimizer):
         gid = torch.full((store.total // 64,), 255, dtype=torch.uint8)
         for gi, p in members:
             off, n, _ = store.offsets[p._vj_name]
-            gid[off // 64:(off + n + 63) // 64] = gi if p.requires_grad else 255   # frozen (pos_embed): untouched
+            gid[off // 64:(off + n + 63) // 64] = gi if self._stepped(p) else 255   # frozen (pos_embed): untouched
         m = torch.zeros(store.total, dtype=torch.float32, device=dev)
         v = torch.zeros(store.total, dtype=torch.float32, device=dev)
         # the step count is a DEVICE scalar (as in torch's fused / capturable AdamW): the kernel advances it only when the
@@ -83,8 +90,8 @@ class FlatAdamW(torch.optim.Optimizer):
                 step.fill_(float(old["step"]))
                 break
         for gi, p in members:
-            if not p.requires_grad:     # torch.optim.AdamW never creates state for a parameter without a gradient (the frozen
-                continue                # pos_embed): keep state_dict() entry-for-entry identical to the reference's
+            if not self._stepped(p):    # torch.optim.AdamW never creates state for a parameter without a gradient (the frozen
+                continue                # pos_embed, the probe's proj): keep state_dict() entry-for-entry identical
             off, n, shape = store.offsets[p._vj_name]
             old = self.state.get(p, {})
             if "exp_avg" in old:
@@ -97,13 +104,12 @@ class FlatAdamW(torch.optim.Optimizer):
 
     @staticmethod
     def _flat_grad_base(store, members):
-        """Device pointer of the flat gradient buffer if every member's .grad is its slice of one buffer."""
+        """Device pointer of the flat gradient buffer if every member's .grad is its slice of one buffer.  Members without
+        a gradient are skipped (not stepped, see _stepped)."""
         base = None
         for _, p in members:
             g = p.grad
             if g is None:
-                if p.requires_grad:
-                    return None
                 continue
             if g.dtype != torch.float32 or not g.is_contiguous():
                 return None

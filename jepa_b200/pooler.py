@@ -3,46 +3,69 @@
 the clip aggregation wrapper (evals/video_classification_frozen/utils.py:86-159).
 
 Same constructor arguments, parameter names, initialisation and `state_dict` keys as the reference, so a probe checkpoint
-written by the reference's eval loop loads here unchanged.  The accelerated path is INFERENCE: `forward` runs under
-no-grad on the hand-written kernels (LayerNorm, wgmma GEMMs with fused bias / GELU / residual epilogues, and
-`vj_cross_attn_fwd` for the query-token attention); training the probe is the evals' job and stays with the reference
-(`forward` raises if a gradient is requested).  There is no CPU fallback.
+written by the reference's eval loop loads here unchanged.  Everything runs on the hand-written kernels (LayerNorm, wgmma
+GEMMs with fused bias / GELU / residual epilogues, `vj_cross_attn_fwd` / `vj_cross_attn_bwd` for the query-token
+attention); there is no CPU fallback.
+
+Training the probe (the frozen evaluations' job, eval.py:317-373): with parameters that require grad, `forward` saves
+what the backward needs and returns outputs with a grad_fn.  The probe's parameters live in one FlatParamStore (fp32
+master weights, bf16 GEMM operands in its shadow) and the backward writes ONE flat fp32 gradient buffer, so FlatAdamW,
+FlatGradScaler and step.clip_grad_norm_ each take one launch over it.  Several probe calls in one step (one per temporal
+segment without attend_across_segments) accumulate into the same buffer.  `proj` gets no gradient: the reference builds
+it but never applies it (modules.py:152-153).  Gradients into the encoder's tokens (fine-tuning) and depth > 1 are not
+implemented.
 """
 import math
+from types import SimpleNamespace
 
 import torch
 import torch.nn as nn
 
 from . import kernels as K
 from .models import MLP
+from .params import FlatParamStore
 from .pos_embs import get_1d_sincos_pos_embed
 from .tensors import apply_masks, trunc_normal_
 
 BF16, F32 = torch.bfloat16, torch.float32
-LN_EPS = 1e-5   # nn.LayerNorm default: AttentivePooler is built with norm_layer=nn.LayerNorm (attentive_pooler.py:30)
 
 
 def _pad_rows(n, mult):
     return (n + mult - 1) // mult * mult
 
 
-class _Shadow:
-    """bf16 copies of the probe's Linear weights (the GEMM B operands), refreshed when a parameter changes."""
+def _store_of(module, anchor):
+    """The FlatParamStore that holds every parameter of `module` (adopting them into module._store if none does) and
+    the name prefix of `module`'s parameters inside it.  A classifier's store holds its pooler too ('pooler.' prefix),
+    so calling clf.pooler directly reuses it instead of moving the parameters."""
+    st = getattr(anchor, "_vj_store", None)
+    if st is None or not all(st.owns(p) for p in module.parameters()):
+        st = module._store.adopt(module)
+    return st, anchor._vj_name[:-len("query_tokens")] if anchor._vj_name.endswith("query_tokens") else ""
 
-    def __init__(self):
-        self._cache = {}
 
-    def get(self, p, pad_rows_to=None):
-        key = id(p)
-        hit = self._cache.get(key)
-        if hit is not None and hit[0] == p._version and hit[1].device == p.device:
-            return hit[1]
-        w = p.detach()
-        if pad_rows_to is not None and w.shape[0] % pad_rows_to:
-            w = torch.cat([w, w.new_zeros(_pad_rows(w.shape[0], pad_rows_to) - w.shape[0], *w.shape[1:])])
-        w = w.to(BF16).contiguous()
-        self._cache[key] = (p._version, w)
-        return w
+def _grad_buffer(store, members):
+    """The flat gradient buffer of this step: the one the members' .grad already alias (an earlier probe call of the
+    same step), else a new zero buffer."""
+    base = None
+    for n, p in members:
+        g = p.grad
+        if g is None or g.dtype != F32 or not g.is_contiguous():
+            base = None
+            break
+        b = g.data_ptr() - 4 * store.offsets[n][0]
+        if base is not None and b != base:
+            base = None
+            break
+        base = b
+    if base is not None:
+        store._grad_gen = getattr(store, "_grad_gen", 0) + 1     # the buffer changes: cached statistics are stale
+        g0 = members[0][1].grad
+        return torch.as_strided(g0, (store.total,), (1,), storage_offset=g0.storage_offset() - store.offsets[members[0][0]][0])
+    gflat = store.new_grad_buffer()
+    for n, p in members:
+        p.grad = store.grad_view(gflat, n)
+    return gflat
 
 
 class CrossAttention(nn.Module):
@@ -94,7 +117,7 @@ class AttentivePooler(nn.Module):
         trunc_normal_(self.query_tokens, std=self.init_std)
         self.apply(self._init_weights)
         self._rescale_blocks()
-        self._shadow = _Shadow()
+        self._store = FlatParamStore()
 
     def _rescale_blocks(self):
         def rescale(param, layer_id):
@@ -115,58 +138,230 @@ class AttentivePooler(nn.Module):
             nn.init.constant_(m.bias, 0)
             nn.init.constant_(m.weight, 1.0)
 
+    def _load_from_state_dict(self, *args, **kwargs):
+        nn.Module._load_from_state_dict(self, *args, **kwargs)
+        _invalidate(self)
+
     def forward(self, x):
         """x [B, S, D] encoder tokens -> pooled query tokens fp32 [B, num_queries, D]."""
-        if torch.is_grad_enabled() and (x.requires_grad or any(p.requires_grad for p in self.parameters())):
-            if x.requires_grad:
-                raise NotImplementedError("the accelerated attentive probe is inference-only: run it under torch.no_grad()")
-        with torch.no_grad():
-            return self._forward(x)
+        return _run_probe(self, self, x, head=False)
 
-    def _forward(self, x):
-        if not x.is_cuda:
-            raise RuntimeError("AttentivePooler: CUDA tensors only (there is no CPU fallback)")
-        B, S, D = x.shape
-        H, nq, dev = self.num_heads, self.num_queries, x.device
-        hd = D // H
-        sh = self._shadow
-        blk = self.cross_attention_block
-        xa = blk.xattn if self.complete_block else blk
-        x2 = x.reshape(B * S, D).contiguous()
-        if x2.dtype not in (BF16, F32):
-            x2 = x2.float()
-        # keys / values: kv(norm1(x)) - one LayerNorm pass and one [B*S, 2D] GEMM (bias in the epilogue)
-        if self.complete_block:
-            xn = torch.empty(B * S, D, dtype=BF16, device=dev)
-            K.layernorm_fwd(x2, xn, blk.norm1.weight.detach().float(), blk.norm1.bias.detach().float(), blk.norm1.eps)
-        else:
-            xn = x2 if x2.dtype == BF16 else x2.to(BF16)
-        kv = torch.empty(B * S, 2 * D, dtype=BF16, device=dev)
-        K.gemm(xn, sh.get(xa.kv.weight), kv, bias=None if xa.kv.bias is None else xa.kv.bias.detach().float())
-        # queries: the learned tokens, identical for every clip -> project once, repeat (rows padded to 8 for 16-byte rows)
-        q0 = self.query_tokens.detach().reshape(nq, D).float()
-        q0b = torch.zeros(_pad_rows(nq, 8), D, dtype=BF16, device=dev)
-        q0b[:nq] = q0.to(BF16)
-        qp = torch.empty(_pad_rows(nq, 8), D, dtype=BF16, device=dev)
-        K.gemm(q0b, sh.get(xa.q.weight), qp, bias=None if xa.q.bias is None else xa.q.bias.detach().float())
-        qrep = qp[:nq].repeat(B, 1).contiguous()                       # [B*nq, D], row b*nq + j = query j of clip b
-        att = torch.empty(B * nq, D, dtype=BF16, device=dev)
-        K.cross_attn_fwd(qrep, kv, att, B, nq, S, H, hd, xa.scale)
-        if not self.complete_block:
-            return att.float().view(B, nq, D)
+
+def _invalidate(module):
+    """Parameters changed behind the optimizer's back (load_state_dict): re-cast the bf16 operands at the next forward."""
+    for p in module.parameters():
+        st = getattr(p, "_vj_store", None)
+        if st is not None:
+            st.invalidate_shadow()
+    module._store.invalidate_shadow()
+
+
+def _run_probe(module, pooler, x, head):
+    if not x.is_cuda:
+        raise RuntimeError("AttentivePooler: CUDA tensors only (there is no CPU fallback)")
+    train = torch.is_grad_enabled() and any(p.requires_grad for p in module.parameters())
+    if torch.is_grad_enabled() and x.requires_grad:
+        raise NotImplementedError("the accelerated attentive probe trains the probe only: gradients into the encoder's "
+                                  "tokens (fine-tuning) are not implemented - pass detached tokens")
+    store, prefix = _store_of(module, pooler.query_tokens)
+    store.refresh_shadow()
+    if not train:
+        with torch.no_grad():
+            y, _ = _probe_forward(pooler, store, prefix, x, head, save=False)
+        return y
+    return _ProbeFn.apply(pooler, store, prefix, x, head, *module.parameters())
+
+
+class _ProbeFn(torch.autograd.Function):
+    """forward: the probe on the kernels, saving its activations.  backward: accumulates every trainable parameter's
+    gradient into the store's flat gradient buffer of this step (and points .grad at its slices) - a flat buffer that two
+    probe calls of one step can share, which autograd's per-tensor accumulation would break apart - and returns None for
+    the parameters.  proj is left without a gradient, as in the reference."""
+
+    @staticmethod
+    def forward(ctx, pooler, store, prefix, x, head, *params):
+        y, sv = _probe_forward(pooler, store, prefix, x, head, save=True)
+        ctx.pooler, ctx.store, ctx.prefix, ctx.sv, ctx.head, ctx.params = pooler, store, prefix, sv, head, params
+        return y
+
+    @staticmethod
+    def backward(ctx, dy):
+        pooler, store, prefix, sv = ctx.pooler, ctx.store, ctx.prefix, ctx.sv
+        members = [(p._vj_name, p) for p in ctx.params if p.requires_grad and ".proj." not in p._vj_name]
+        if members:
+            gflat = _grad_buffer(store, members)
+            _probe_backward(pooler, store, prefix, sv, dy, ctx.head, gflat)
+        n = len(ctx.params)
+        ctx.sv = ctx.params = None
+        return (None, None, None, None, None) + (None,) * n
+
+
+def _names(pooler, prefix):
+    blk = prefix + "cross_attention_block."
+    return blk, (blk + "xattn." if pooler.complete_block else blk)
+
+
+def _probe_forward(pooler, store, prefix, x, head, save):
+    """Pooler (+ linear head) forward.  Returns (pooled fp32 [B, nq, D] or logits fp32 [B, C], saved activations)."""
+    B, S, D = x.shape
+    H, nq, dev = pooler.num_heads, pooler.num_queries, x.device
+    hd = D // H
+    blk, xa = _names(pooler, prefix)
+    w = store.bf16
+    f = store.f32
+    has_qkv_bias = (xa + "kv.bias") in store.offsets
+    x2 = x.detach().reshape(B * S, D).contiguous()
+    if x2.dtype not in (BF16, F32):
+        x2 = x2.float()
+    sv = SimpleNamespace(B=B, S=S, x2=x2) if save else None
+    # keys / values: kv(norm1(x)) - one LayerNorm pass and one [B*S, 2D] GEMM (bias in the epilogue)
+    if pooler.complete_block:
+        xn = torch.empty(B * S, D, dtype=BF16, device=dev)
+        mean1 = torch.empty(B * S, dtype=F32, device=dev) if save else None
+        rstd1 = torch.empty(B * S, dtype=F32, device=dev) if save else None
+        K.layernorm_fwd(x2, xn, f(blk + "norm1.weight"), f(blk + "norm1.bias"), pooler.cross_attention_block.norm1.eps,
+                        mean1, rstd1)
+    else:
+        xn = x2 if x2.dtype == BF16 else x2.to(BF16)
+        mean1 = rstd1 = None
+    kv = torch.empty(B * S, 2 * D, dtype=BF16, device=dev)
+    K.gemm(xn, w(xa + "kv.weight"), kv, bias=f(xa + "kv.bias") if has_qkv_bias else None)
+    # queries: the learned tokens, identical for every clip -> project once, repeat (rows padded to 8 for 16-byte rows)
+    q0 = f(prefix + "query_tokens").reshape(nq, D)
+    q0b = torch.zeros(_pad_rows(nq, 8), D, dtype=BF16, device=dev)
+    q0b[:nq] = q0.to(BF16)
+    qp = torch.empty(_pad_rows(nq, 8), D, dtype=BF16, device=dev)
+    K.gemm(q0b, w(xa + "q.weight"), qp, bias=f(xa + "q.bias") if has_qkv_bias else None)
+    qrep = qp[:nq].repeat(B, 1).contiguous()                       # [B*nq, D], row b*nq + j = query j of clip b
+    att = torch.empty(B * nq, D, dtype=BF16, device=dev)
+    if save:
+        lse2 = torch.empty(B * nq, H, dtype=F32, device=dev)
+        K.cross_attn_fwd_lse(qrep, kv, att, lse2, B, nq, S, H, hd, pooler.cross_attention_block.xattn.scale
+                             if pooler.complete_block else pooler.cross_attention_block.scale)
+        sv.xn, sv.mean1, sv.rstd1, sv.kv, sv.q0b, sv.qrep, sv.att, sv.lse2 = xn, mean1, rstd1, kv, q0b, qrep, att, lse2
+    else:
+        K.cross_attn_fwd(qrep, kv, att, B, nq, S, H, hd, pooler.cross_attention_block.xattn.scale
+                         if pooler.complete_block else pooler.cross_attention_block.scale)
+    M = _pad_rows(B * nq, 8)
+    if not pooler.complete_block:
+        pooled = att.float()
+    else:
         # q = q + y ; q = q + fc2(gelu(fc1(norm2(q))))   (fp32 residual stream: it is only B*nq rows)
-        q1 = q0.repeat(B, 1) + att.float()
-        M = _pad_rows(B * nq, 8)
         q1p = torch.zeros(M, D, dtype=F32, device=dev)
-        q1p[:B * nq] = q1
+        q1p[:B * nq] = q0.repeat(B, 1) + att.float()
         ln2 = torch.empty(M, D, dtype=BF16, device=dev)
-        K.layernorm_fwd(q1p, ln2, blk.norm2.weight.detach().float(), blk.norm2.bias.detach().float(), blk.norm2.eps)
-        hid = blk.mlp.fc1.weight.shape[0]
+        mean2 = torch.empty(M, dtype=F32, device=dev) if save else None
+        rstd2 = torch.empty(M, dtype=F32, device=dev) if save else None
+        K.layernorm_fwd(q1p, ln2, f(blk + "norm2.weight"), f(blk + "norm2.bias"), pooler.cross_attention_block.norm2.eps,
+                        mean2, rstd2)
+        hid = store.offsets[blk + "mlp.fc1.weight"][2][0]
         g = torch.empty(M, hid, dtype=BF16, device=dev)
-        K.gemm(ln2, sh.get(blk.mlp.fc1.weight), g, bias=blk.mlp.fc1.bias.detach().float(), epi=K.EPI_GELU)
+        # training keeps gelu'(pre-activation) from the same epilogue: the fc1 dgrad is then a plain multiply
+        h = torch.empty(M, hid, dtype=BF16, device=dev) if save else None
+        K.gemm(ln2, w(blk + "mlp.fc1.weight"), g, bias=f(blk + "mlp.fc1.bias"), epi=K.EPI_GELU_GRAD if save else K.EPI_GELU,
+               aux_out=h)
         q2 = torch.empty(M, D, dtype=F32, device=dev)
-        K.gemm(g, sh.get(blk.mlp.fc2.weight), q2, bias=blk.mlp.fc2.bias.detach().float(), epi=K.EPI_ADD, aux=q1p)
-        return q2[:B * nq].view(B, nq, D)
+        K.gemm(g, w(blk + "mlp.fc2.weight"), q2, bias=f(blk + "mlp.fc2.bias"), epi=K.EPI_ADD, aux=q1p)
+        pooled = q2[:B * nq]
+        if save:
+            sv.q1p, sv.ln2, sv.mean2, sv.rstd2, sv.h, sv.g = q1p, ln2, mean2, rstd2, h, g
+    if not head:
+        return pooled.view(B, nq, D), sv
+    # linear head as logits^T [C, Np] = W [C, D] . pooled^T: the GEMM's N is the (padded) batch, so the weight is read
+    # straight from the store for any class count; the bias comes in through the residual epilogue
+    C = store.offsets["linear.weight"][2][0]
+    Np = _pad_rows(B, 64)
+    pb = torch.zeros(Np, D, dtype=BF16, device=dev)
+    pb[:B] = pooled
+    bias_t = f("linear.bias").unsqueeze(1).expand(C, Np).contiguous()
+    lt = torch.empty(C, Np, dtype=F32, device=dev)
+    K.gemm(w("linear.weight"), pb, lt, epi=K.EPI_ADD, aux=bias_t)
+    if save:
+        sv.pb = pb
+    return lt[:, :B].t().contiguous(), sv
+
+
+def _probe_backward(pooler, store, prefix, sv, dy, head, gflat):
+    B, S, D = sv.B, sv.S, sv.x2.shape[1]
+    H, nq, dev = pooler.num_heads, pooler.num_queries, gflat.device
+    hd = D // H
+    blk, xa = _names(pooler, prefix)
+    w = store.bf16
+    f = store.f32
+    gv = lambda name: store.grad_view(gflat, name)
+    has_qkv_bias = (xa + "kv.bias") in store.offsets
+    M, Mp = B * nq, _pad_rows(B * nq, 8)
+    if head:
+        # dlogits [B, C] -> dW += dlogits^T pooled, db += column sums, dpooled = dlogits W
+        C = store.offsets["linear.weight"][2][0]
+        Np = sv.pb.shape[0]
+        dl = dy.detach().to(F32)
+        dlt = torch.zeros(C, Np, dtype=BF16, device=dev)
+        dlt[:, :B] = dl.t()
+        K.gemm(dlt, sv.pb, gv("linear.weight"), b_mn=True, accumulate=True)
+        Cp = _pad_rows(C, 8)      # colsum works on 8-column groups: the bias slice is followed by store padding
+        dlp = torch.zeros(B, Cp, dtype=F32, device=dev)
+        dlp[:, :C] = dl
+        boff = store.offsets["linear.bias"][0]
+        K.colsum(dlp, gflat[boff:boff + Cp])
+        dpooled = torch.empty(Np, D, dtype=F32, device=dev)
+        K.gemm(dlt, w("linear.weight"), dpooled, a_mn=True, b_mn=True)
+        dq2 = torch.zeros(Mp, D, dtype=F32, device=dev)
+        dq2[:M] = dpooled[:B]
+    else:
+        dq2 = torch.zeros(Mp, D, dtype=F32, device=dev)
+        dq2[:M] = dy.detach().reshape(M, D)
+    if pooler.complete_block:
+        # MLP: q2 = q1 + fc2(gelu(fc1(ln2(q1))))
+        dq2b = dq2.to(BF16)
+        _wgrad(dq2b, sv.g, gv(blk + "mlp.fc2.weight"), gv(blk + "mlp.fc2.bias"), Mp)
+        hid = sv.g.shape[1]
+        dpre = torch.empty(Mp, hid, dtype=BF16, device=dev)
+        K.gemm(dq2b, w(blk + "mlp.fc2.weight"), dpre, b_mn=True, epi=K.EPI_MUL, aux=sv.h)
+        _wgrad(dpre, sv.ln2, gv(blk + "mlp.fc1.weight"), gv(blk + "mlp.fc1.bias"), Mp)
+        dln2 = torch.empty(Mp, D, dtype=BF16, device=dev)
+        K.gemm(dpre, w(blk + "mlp.fc1.weight"), dln2, b_mn=True)
+        dq1 = torch.empty(Mp, D, dtype=F32, device=dev)
+        K.layernorm_bwd(dln2, sv.q1p, f(blk + "norm2.weight"), sv.mean2, sv.rstd2, dq2, dq1, gv(blk + "norm2.weight"),
+                        gv(blk + "norm2.bias"))
+    else:
+        dq1 = dq2
+    # cross-attention
+    datt = dq1[:M].to(BF16)
+    dqrep = torch.empty(M, D, dtype=F32, device=dev)
+    dkv = torch.empty(B * S, 2 * D, dtype=BF16, device=dev)
+    scale = pooler.cross_attention_block.xattn.scale if pooler.complete_block else pooler.cross_attention_block.scale
+    K.cross_attn_bwd(sv.qrep, sv.kv, sv.att, datt, sv.lse2, dqrep, dkv, B, nq, S, H, hd, scale)
+    # the query projection is shared by all clips: sum its gradient over them (row b*nq + j -> query j)
+    dqp = torch.zeros(_pad_rows(nq, 8), D, dtype=F32, device=dev)
+    gq = gv(prefix + "query_tokens").view(nq, D)
+    for j in range(nq):
+        K.colsum(dqrep, dqp[j], period=nq, lo=j, hi=j + 1)
+        if pooler.complete_block:      # residual path q1 = q0 + y
+            K.colsum(dq1[:M], gq[j], period=nq, lo=j, hi=j + 1)
+    dqpb = dqp.to(BF16)
+    _wgrad(dqpb, sv.q0b, gv(xa + "q.weight"), None, dqpb.shape[0])
+    if has_qkv_bias:
+        K.colsum(dqp, gv(xa + "q.bias"))
+    K.gemm(dqpb[:nq], w(xa + "q.weight"), gq, b_mn=True, accumulate=True)
+    # keys / values: kv = xn W_kv^T + b over all B*S tokens
+    _wgrad(dkv, sv.xn, gv(xa + "kv.weight"), gv(xa + "kv.bias") if has_qkv_bias else None, B * S)
+    if pooler.complete_block:
+        # norm1's affine parameters only: the gradient into the frozen encoder's tokens goes to scratch
+        dxn = torch.empty(B * S, D, dtype=BF16, device=dev)
+        K.gemm(dkv, w(xa + "kv.weight"), dxn, b_mn=True)
+        dx = torch.empty_like(sv.x2)
+        K.layernorm_bwd(dxn, sv.x2, f(blk + "norm1.weight"), sv.mean1, sv.rstd1, None, dx, gv(blk + "norm1.weight"),
+                        gv(blk + "norm1.bias"))
+
+
+def _wgrad(dy, act, grad_out, bias_grad, tokens):
+    """grad_out[N_out, K_in] += dy^T act over `tokens` rows; bias_grad[N_out] += colsum(dy).  One CTA per output tile
+    (split_k = 1: no reduce-add of split pieces, so the weight gradients are bitwise reproducible); the probe's weight
+    gradients have 64 .. 256 output tiles, which fills the GPU without splitting the token range."""
+    K.gemm(dy, act, grad_out, a_mn=True, b_mn=True, accumulate=True, split_k=1)
+    if bias_grad is not None:
+        K.colsum(dy, bias_grad)
 
 
 class AttentiveClassifier(nn.Module):
@@ -179,21 +374,15 @@ class AttentiveClassifier(nn.Module):
                                       depth=depth, norm_layer=norm_layer, init_std=init_std, qkv_bias=qkv_bias,
                                       complete_block=complete_block)
         self.linear = nn.Linear(embed_dim, num_classes, bias=True)
-        self._shadow = _Shadow()
+        self._store = FlatParamStore()
+
+    def _load_from_state_dict(self, *args, **kwargs):
+        nn.Module._load_from_state_dict(self, *args, **kwargs)
+        _invalidate(self)
 
     def forward(self, x):
-        pooled = self.pooler(x).squeeze(1)                              # [B, D] fp32
-        with torch.no_grad():
-            B, D = pooled.shape
-            C = self.linear.out_features
-            M, Cp = _pad_rows(B, 8), _pad_rows(C, 64)                   # GEMM N must be a multiple of 64: zero weight rows
-            a = torch.zeros(M, D, dtype=BF16, device=pooled.device)
-            a[:B] = pooled.to(BF16)
-            bias = torch.zeros(Cp, dtype=F32, device=pooled.device)
-            bias[:C] = self.linear.bias.detach().float()
-            out = torch.empty(M, Cp, dtype=F32, device=pooled.device)
-            K.gemm(a, self._shadow.get(self.linear.weight, pad_rows_to=64), out, bias=bias)
-            return out[:B, :C]
+        """x [B, S, D] encoder tokens -> logits fp32 [B, num_classes]."""
+        return _run_probe(self, self.pooler, x, head=True)
 
 
 class ClipAggregation(nn.Module):

@@ -171,7 +171,7 @@ def clip_grad_norm_(module, max_norm):
     if flat is None or len(flat) != len(named):
         return torch.nn.utils.clip_grad_norm_([p for _, p in named], max_norm)
     sumsq = next(iter(flat.values()))[0]
-    store = bb._store
+    store = named[0][1]._vj_store
     out = torch.empty(2, dtype=torch.float32, device=sumsq.device)
     K.clip_coef(sumsq, max_norm, out[0:1], out[1:2])
     p0 = named[0][1]
