@@ -219,6 +219,17 @@ int vj_sumsq(const float* x, long long n, float* out, void* stream);
 int vj_clip_preprocess(const void* src_u8, const void* params, void* out, int out_f32, int B, int T, int S,
                        const float* mean3, const float* std3, void* stream);
 
+/* Deterministic evaluation views: uint8 frames -> OpenCV INTER_LINEAR short-side resize (bit-exact fixed point) ->
+ * S x S window -> / 255 -> (x - mean) / std -> fp32 or bf16 [3, T, S, S] per view, one launch for every (clip, segment,
+ * view).  jobs: device table, one 32-byte record per view = {int64 byte offset of the clip in src_u8, int64 element
+ * offset of the view in out, int32 H, W, ytab, xtab}; tab: device int4 table (source index 0, source index 1, weight 0,
+ * weight 1) per resized row / column, OpenCV's 11-bit weights, S consecutive entries from ytab (rows) and xtab
+ * (columns) per view.  mean3 / std3: HOST arrays of 3 floats.  Replaces EvalVideoTransform and
+ * VideoTransform(training=False) of evals/video_classification_frozen/utils.py; the geometry and the tables come from
+ * jepa_b200/transforms.py. */
+int vj_clip_views(const void* src_u8, const void* jobs, const void* tab, void* out, int out_f32, int n_jobs, int T, int S,
+                  const float* mean3, const float* std3, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

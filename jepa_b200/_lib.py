@@ -19,6 +19,7 @@ SIGNATURES = {
     "vj_tmap_cache_stats": (L, [I]),
     "vj_set_sm_limit": (I, [I]),
     "vj_clip_preprocess": (I, [P, P, P, I, I, I, I, P, P, P]),
+    "vj_clip_views": (I, [P, P, P, P, I, I, I, I, P, P, P]),
     "vj_gemm": (I, [P, L, I, P, L, I, P, L, I, I, I, I, P, F, I, P, L, I, P, I, P, L, I, I, P]),
     "vj_attn_fwd": (I, [P, P, P, P, I, I, I, I, I, F, P]),
     "vj_attn_bwd": (I, [P, P, P, P, P, P, P, P, I, I, I, I, I, F, P]),

@@ -203,10 +203,41 @@ class FlatGradSync:
             _wait_pending()
 
 
+class ProbeGradSync:
+    """Gradient exchange of a trainable attentive probe (jepa_b200.pooler): ONE averaging all-reduce of the probe's whole
+    flat fp32 gradient buffer per backward pass, issued from an end-of-backward callback.  The probe's backward writes
+    that buffer in one piece (no per-layer readiness to overlap with), and several probe calls of one step (one per
+    temporal segment without attend_across_segments) add into the same buffer first, so they are exchanged once."""
+
+    def __init__(self, process_group=None):
+        self.group = process_group
+        self.gflat = None
+        self.n_calls = 0    # all-reduces issued (tests)
+
+    def mark(self, gflat):
+        """Called by every probe backward with the buffer it accumulated into.  Each call queues an end-of-backward
+        callback; the first one to run exchanges the buffer and the others find nothing left to do, so a pass issues
+        exactly one all-reduce (and a backward that raised part-way leaves nothing armed for the next one)."""
+        self.gflat = gflat
+        torch.autograd.Variable._execution_engine.queue_callback(self._exchange)
+
+    def _exchange(self):
+        g, self.gflat = self.gflat, None
+        if g is None or not _active():
+            return
+        if dist.get_backend(self.group) == 'nccl':
+            dist.all_reduce(g, op=dist.ReduceOp.AVG, group=self.group)
+        else:  # gloo (CPU tests): no AVG
+            g.div_(dist.get_world_size(self.group))
+            dist.all_reduce(g, op=dist.ReduceOp.SUM, group=self.group)
+        self.n_calls += 1
+
+
 class DistributedDataParallel(torch.nn.Module):
     """Data-parallel wrapper with torch DDP's surface (`.module`, `module.`-prefixed state dict, forward passthrough,
     parameters broadcast from rank 0 at construction) whose gradient exchange is FlatGradSync on the flat gradient
-    buffers instead of reducer buckets.  Frozen modules (the target encoder) only get the broadcast."""
+    buffers instead of reducer buckets (encoder / predictor), or ProbeGradSync for an attentive probe (a module with a
+    flat store but no layer-stack spec).  Frozen modules (the target encoder) only get the broadcast."""
 
     def __init__(self, module, device_ids=None, static_graph=False, process_group=None, bucket_cap_mb=96, **_ignored):
         super().__init__()
@@ -217,9 +248,14 @@ class DistributedDataParallel(torch.nn.Module):
                 for t in list(module.parameters()) + list(module.buffers()):
                     dist.broadcast(t.data, 0, group=process_group)
             if any(p.requires_grad for p in module.parameters()):
+                probe_sync = None
                 for m in module.modules():
                     if hasattr(m, '_store') and hasattr(m, '_spec'):
                         m._vj_grad_sync = FlatGradSync(process_group, bucket_cap_mb << 20)
+                    elif hasattr(m, '_store'):
+                        # a classifier and its pooler share one store (and one buffer): one exchange object for both
+                        probe_sync = probe_sync or ProbeGradSync(process_group)
+                        m._vj_probe_sync = probe_sync
 
     def forward(self, *args, **kwargs):
         return self.module(*args, **kwargs)

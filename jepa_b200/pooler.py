@@ -156,7 +156,18 @@ def _invalidate(module):
     module._store.invalidate_shadow()
 
 
+def _inside_torch_ddp(module):
+    """True while torch's own DistributedDataParallel runs `module`'s forward.  Its reducer waits for per-parameter
+    gradient hooks, which the probe's flat-buffer backward never fires, so the replicas would silently drift apart."""
+    active = getattr(torch.nn.parallel.DistributedDataParallel, "_active_ddp_module", None)
+    return active is not None and getattr(active, "module", None) is module
+
+
 def _run_probe(module, pooler, x, head):
+    if _inside_torch_ddp(module):
+        raise NotImplementedError("the attentive probe cannot be wrapped in torch.nn.parallel.DistributedDataParallel "
+                                  "(its backward writes one flat gradient buffer and never fires the reducer's hooks); "
+                                  "wrap it in src.utils.distributed.DistributedDataParallel")
     if not x.is_cuda:
         raise RuntimeError("AttentivePooler: CUDA tensors only (there is no CPU fallback)")
     train = torch.is_grad_enabled() and any(p.requires_grad for p in module.parameters())
@@ -169,7 +180,7 @@ def _run_probe(module, pooler, x, head):
         with torch.no_grad():
             y, _ = _probe_forward(pooler, store, prefix, x, head, save=False)
         return y
-    return _ProbeFn.apply(pooler, store, prefix, x, head, *module.parameters())
+    return _ProbeFn.apply(pooler, store, prefix, x, head, getattr(module, "_vj_probe_sync", None), *module.parameters())
 
 
 class _ProbeFn(torch.autograd.Function):
@@ -179,9 +190,10 @@ class _ProbeFn(torch.autograd.Function):
     the parameters.  proj is left without a gradient, as in the reference."""
 
     @staticmethod
-    def forward(ctx, pooler, store, prefix, x, head, *params):
+    def forward(ctx, pooler, store, prefix, x, head, sync, *params):
         y, sv = _probe_forward(pooler, store, prefix, x, head, save=True)
         ctx.pooler, ctx.store, ctx.prefix, ctx.sv, ctx.head, ctx.params = pooler, store, prefix, sv, head, params
+        ctx.sync = sync
         return y
 
     @staticmethod
@@ -191,9 +203,11 @@ class _ProbeFn(torch.autograd.Function):
         if members:
             gflat = _grad_buffer(store, members)
             _probe_backward(pooler, store, prefix, sv, dy, ctx.head, gflat)
+            if ctx.sync is not None:       # data parallel: average the buffer once, at the end of this backward pass
+                ctx.sync.mark(gflat)
         n = len(ctx.params)
-        ctx.sv = ctx.params = None
-        return (None, None, None, None, None) + (None,) * n
+        ctx.sv = ctx.params = ctx.sync = None
+        return (None, None, None, None, None, None) + (None,) * n
 
 
 def _names(pooler, prefix):
