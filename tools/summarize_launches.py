@@ -13,16 +13,19 @@ def family(name):
     m = re.search(r"vj::(\w+)", name)
     if m:
         k = m.group(1)
-        if k == "gemm_kernel":
-            t = re.search(r"gemm_kernel<([^>]*)>", name)
+        if k in ("gemm_kernel", "gemm_wgrad_kernel"):
+            # gemm_kernel<BN, COOP, B_MN, OUT_F32, EPI, AUX32> (forward / dgrad: ping-pong, or cooperative for long K)
+            # gemm_wgrad_kernel<BN, OUT_F32> (weight gradients: both operands MN-major, cooperative, no epilogue op)
+            t = re.search(k + r"<([^>]*)>", name)
             a = [x.strip().replace("(bool)", "").replace("(int)", "") for x in t.group(1).split(",")] if t else []
-            if len(a) == 6:
-                a.append("0")
-            if len(a) == 7:
-                yes = lambda x: x in ("1", "true")
-                major = "MN-MN" if yes(a[1]) and yes(a[2]) else ("K-MN" if yes(a[2]) else "KK")
+            yes = lambda x: x in ("1", "true")
+            if k == "gemm_kernel" and len(a) == 6:
+                sched = "coop" if yes(a[1]) else "pingpong"
                 epi = {"0": "none", "1": "gelu", "2": "add", "3": "dgelu", "4": "mul", "5": "gelu+grad"}.get(a[4], a[4])
-                return f"gemm {major} bn{a[0]} {epi}{' f32out' if yes(a[3]) else ''}{' aux32' if yes(a[5]) else ''}{' ring' if yes(a[6]) else ''}"
+                return (f"gemm {'K-MN' if yes(a[2]) else 'KK'} {sched} bn{a[0]} {epi}"
+                        f"{' f32out' if yes(a[3]) else ''}{' aux32' if yes(a[5]) else ''}")
+            if k == "gemm_wgrad_kernel" and len(a) == 2:
+                return f"gemm MN-MN coop bn{a[0]} none{' f32out' if yes(a[1]) else ''}"
         t = re.search(r"vj::(\w+)<([^>]*)>", name)
         return f"{k}<{t.group(2)}>" if t else k
     if "nccl" in name.lower():
