@@ -28,7 +28,7 @@ from app.vjepa.transforms import make_transforms
 from app.vjepa.utils import init_opt, init_video_model, load_checkpoint
 from jepa_b200 import step as vj
 from jepa_b200.checkpoint import AsyncCheckpointer
-from jepa_b200.transforms import preprocess_batch
+from jepa_b200.transforms import tickets_to_device
 from src.datasets.data_manager import init_data
 from src.masks.multiblock3d import MaskCollator as MB3DMaskCollator
 from src.masks.random_tube import MaskCollator as TubeMaskCollator
@@ -103,6 +103,7 @@ def main(args, resume_preempt=False):
     motion_shift = aug.get('motion_shift', False)
     reprob = aug.get('reprob', 0.)
     use_aa = aug.get('auto_augment', False)
+    gpu_augment = aug.get('gpu_augment', False)     # RandAugment / random erasing on the GPU
 
     loss_cfg = args.get('loss')
     loss_exp = loss_cfg.get('loss_exp')
@@ -169,7 +170,7 @@ def main(args, resume_preempt=False):
                                  tubelet_size=tubelet_size, cfgs_mask=cfgs_mask)
     transform = make_transforms(random_horizontal_flip=True, random_resize_aspect_ratio=ar_range,
                                 random_resize_scale=rr_scale, reprob=reprob, auto_augment=use_aa,
-                                motion_shift=motion_shift, crop_size=crop_size)
+                                motion_shift=motion_shift, crop_size=crop_size, gpu_augment=gpu_augment)
 
     (unsupervised_loader, unsupervised_sampler) = init_data(
         data=dataset_type, root_path=dataset_paths, batch_size=batch_size, training=True, clip_len=num_frames,
@@ -266,8 +267,8 @@ def main(args, resume_preempt=False):
 
             # host -> device; every clip of a sample reuses that sample's mask pair (train.py:391-409)
             def to_device(u):
-                if isinstance(u, (list, tuple)):   # ClipTickets: uint8 frames cross PCIe, one kernel crops / flips / normalises
-                    return preprocess_batch(list(u), device, crop_size)
+                if isinstance(u, (list, tuple)):   # tickets: uint8 frames cross PCIe, the kernels augment / crop / normalise
+                    return tickets_to_device(list(u), device, crop_size)
                 return u.to(device, non_blocking=True)
             clips = torch.cat([to_device(u) for u in udata[0]], dim=0)
             masks_enc = [repeat_interleave_batch(m.to(device, non_blocking=True), batch_size, repeat=num_clips)

@@ -30,7 +30,7 @@ import torch.nn.functional as F
 import src.models.vision_transformer as vit
 from evals.video_classification_frozen.utils import ClipAggregation, FrameAggregation, make_transforms
 from jepa_b200.optim import FlatAdamW, FlatGradScaler
-from jepa_b200.transforms import GpuEvalVideoTransform
+from jepa_b200.transforms import GpuEvalVideoTransform, GpuVideoTransform
 from src.datasets.data_manager import init_data
 from src.models.attentive_pooler import AttentiveClassifier
 from src.utils.distributed import AllReduce, DistributedDataParallel, init_distributed
@@ -84,6 +84,7 @@ def main(args_eval, resume_preempt=False):
     eval_duration = args_pretrain.get('clip_duration', None)
     eval_num_views_per_segment = args_data.get('num_views_per_segment', 1)
     synthetic_length = args_data.get('synthetic_length', None)     # synthetic datasets only: items per split
+    gpu_augment = args_data.get('gpu_augment', False)     # training transform (RandAugment, erasing) on the GPU
 
     args_opt = args_eval.get('optimization')
     resolution = args_opt.get('resolution', 224)
@@ -144,7 +145,7 @@ def main(args_eval, resume_preempt=False):
                                    num_segments=eval_num_segments if attend_across_segments else 1,
                                    num_views_per_segment=1, allow_segment_overlap=True, batch_size=batch_size,
                                    world_size=world_size, rank=rank, training=True, num_classes=num_classes,
-                                   synthetic_length=synthetic_length)
+                                   synthetic_length=synthetic_length, gpu_augment=gpu_augment)
     val_loader = make_dataloader(dataset_type=dataset_type, root_path=val_data_path, resolution=resolution,
                                  frames_per_clip=eval_frames_per_clip, frame_step=eval_frame_step,
                                  num_segments=eval_num_segments, eval_duration=eval_duration,
@@ -200,10 +201,15 @@ def main(args_eval, resume_preempt=False):
 
 def load_clips(data, device, data_loader):
     """data[0] (segments of views, collated) -> device.  uint8 frames from a loader whose dataset carries the GPU
-    evaluation transform become the reference's views through vj_clip_views; pre-normalised views are copied."""
+    evaluation transform become the reference's views through vj_clip_views; training tickets of every segment go
+    through one augment_batch (RandAugment, crop, erase); pre-normalised views are copied."""
     transform = getattr(getattr(data_loader, 'dataset', None), 'transform', None)
     if isinstance(transform, GpuEvalVideoTransform):
         return transform.views(data[0], device)
+    if isinstance(transform, GpuVideoTransform):
+        B = len(data[0][0])
+        out = transform.batch([t for seg in data[0] for t in seg], device)
+        return [[out[s * B:(s + 1) * B]] for s in range(len(data[0]))]
     return [[dij.to(device, non_blocking=True) for dij in di] for di in data[0]]
 
 
@@ -321,9 +327,10 @@ def load_pretrained(encoder, pretrained, checkpoint_key='target_encoder'):
 def make_dataloader(root_path, batch_size, world_size, rank, dataset_type='VideoDataset', resolution=224,
                     frames_per_clip=16, frame_step=4, num_segments=8, eval_duration=None, num_views_per_segment=1,
                     allow_segment_overlap=True, training=False, num_workers=12, subset_file=None, num_classes=None,
-                    synthetic_length=None):
-    """eval.py:442-488.  The training transform keeps the reference's arguments (RandAugment, random erasing), so it
-    raises for uint8 inputs; the synthetic dataset is pre-normalised and needs no transform.  num_classes /
+                    synthetic_length=None, gpu_augment=False):
+    """eval.py:442-488.  The training transform keeps the reference's arguments (RandAugment, random erasing): with
+    gpu_augment it runs on the GPU, without it it raises for uint8 inputs; the synthetic dataset is pre-normalised and
+    needs no transform.  num_classes /
     synthetic_length select the labelled synthetic evaluation items of src.datasets.data_manager."""
     kind = str(dataset_type).lower()
     transform = None
@@ -331,7 +338,7 @@ def make_dataloader(root_path, batch_size, world_size, rank, dataset_type='Video
         transform = make_transforms(training=training, num_views_per_clip=num_views_per_segment,
                                     random_horizontal_flip=False, random_resize_aspect_ratio=(0.75, 4 / 3),
                                     random_resize_scale=(0.08, 1.0), reprob=0.25, auto_augment=True, motion_shift=False,
-                                    crop_size=resolution)
+                                    crop_size=resolution, gpu_augment=gpu_augment)
     if kind.startswith('synthetic'):
         num_workers = 0          # items are generated in-process
     data_loader, _ = init_data(data=dataset_type, root_path=root_path, transform=transform, batch_size=batch_size,

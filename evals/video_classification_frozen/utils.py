@@ -1,7 +1,8 @@
 """Import path of the reference (evals/video_classification_frozen/utils.py): the clip aggregation wrapper and the
 evaluation transforms.  make_transforms(training=False) returns the GPU evaluation transform: the frames stay uint8
 through the loader and vj_clip_views makes the EvalVideoTransform / VideoTransform(training=False) views on the device.
-The training transform (RandAugment + random erasing in every shipped config) raises - see jepa_b200.transforms."""
+The training transform (RandAugment + random erasing in every shipped config) runs on the GPU with gpu_augment=True
+and raises without it - see jepa_b200.transforms."""
 import torch.nn as nn
 
 from jepa_b200.pooler import ClipAggregation  # noqa: F401

@@ -230,6 +230,24 @@ int vj_clip_preprocess(const void* src_u8, const void* params, void* out, int ou
 int vj_clip_views(const void* src_u8, const void* jobs, const void* tab, void* out, int out_f32, int n_jobs, int T, int S,
                   const float* mean3, const float* std3, void* stream);
 
+/* Training transform with RandAugment and random erasing: uint8 frames -> n_layers RandAugment layers (PIL 12
+ * arithmetic, bit-exact) -> random-resized crop (bilinear) -> flip -> (x - 255 mean) / (255 std) -> erase box filled
+ * with N(0, 1) (Philox keyed by the clip's seed) -> fp32 or bf16 [B, 3, T, S, S].
+ * buf0 / buf1: two device uint8 work buffers of equal size; buf0 holds the frames on entry, both are overwritten.
+ * clips: device table, one 64-byte record per clip = {int64 byte offset of the clip [T, H, W, 3] in each buffer, int32 H,
+ * W, i, j, h, w (crop box), flip, final_buf (buffer holding the clip after the last layer), erase top, left, h, w (h 0:
+ * no erase), uint64 seed}.  ops: device table [n_layers, B] of 64-byte records = {double inverse affine matrix[6],
+ * int32 op (index in jepa_b200.transforms.RA_OPS, -1 skipped), float factor, int32 argument, int32 input buffer}.
+ * hist: device int32 scratch of n_layers * B * T * 1024.  layer_flags: HOST int[n_layers], bit 0: some op applied,
+ * bit 1: some op reads the frame histogram.  mean3 / std3: HOST arrays of 3 floats.  At most 2 launches per layer + 1.
+ * Replaces src/datasets/utils/video/randaugment.py:51-180 / :324-465 (RandAugment on PIL frames),
+ * src/datasets/utils/video/randerase.py:116-156 (RandomErasing._erase_cube, mode 'pixel') and the training paths of
+ * app/vjepa/transforms.py:86-115 and evals/video_classification_frozen/utils.py:251-283; the decisions come from
+ * jepa_b200/transforms.py. */
+int vj_clip_augment(void* buf0, void* buf1, const void* clips, const void* ops, void* hist, const int* layer_flags,
+                    int n_layers, void* out, int out_f32, int B, int T, int S, const float* mean3, const float* std3,
+                    void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -15,19 +15,10 @@
 // out : [B, 3, T, S, S] fp32 or bf16 (the Conv3d / vj_im2col_tubelets input layout)
 // Bilinear sampling follows ATen's upsample_bilinear2d (align_corners = False): src = max(0, (dst + 0.5) * in/out - 0.5),
 // the upper neighbour is clamped to the last row / column of the CROP.
-#include "common.cuh"
+#include "preprocess.cuh"
 #include "vjepa_b200.h"
 
 namespace vj {
-
-// (v_c - sub_c) / div_c for the three channels, each step rounded like the reference's fp32 sub_ / div_, stored as TO
-// at dst + c * cstride (the channel planes of the [3, T, S, S] layout)
-template <typename TO>
-__device__ __forceinline__ void normalise_store(TO* dst, long long cstride, const float (&v)[3], float3 sub, float3 div) {
-  dst[0] = TO(__fdiv_rn(__fsub_rn(v[0], sub.x), div.x));
-  dst[cstride] = TO(__fdiv_rn(__fsub_rn(v[1], sub.y), div.y));
-  dst[2 * cstride] = TO(__fdiv_rn(__fsub_rn(v[2], sub.z), div.z));
-}
 
 struct ClipParam {     // one per clip, 8 x int32 + 1 x int64 offset (host-built, device-resident)
   long long src_off;   // byte offset of the clip's first frame in `src`
@@ -50,21 +41,8 @@ __global__ void __launch_bounds__(256) clip_preprocess_kernel(const uint8_t* __r
   for (int idx = blockIdx.x * blockDim.x + threadIdx.x; idx < S * S; idx += gridDim.x * blockDim.x) {
     const int y = idx / S, xo = idx - y * S;
     const int x = cp.flip ? (S - 1 - xo) : xo;              // output column xo shows resized column x
-    float fy = fmaxf((float(y) + 0.5f) * sh - 0.5f, 0.f);
-    float fx = fmaxf((float(x) + 0.5f) * sw - 0.5f, 0.f);
-    const int y0 = min(int(fy), cp.h - 1), x0 = min(int(fx), cp.w - 1);
-    const int y1 = min(y0 + 1, cp.h - 1), x1 = min(x0 + 1, cp.w - 1);
-    const float ly = fy - float(y0), lx = fx - float(x0);
-    const float hy = 1.f - ly, hx = 1.f - lx;
-    const uint8_t* r0 = frame + ((long long)(cp.i + y0) * cp.W + cp.j) * 3;
-    const uint8_t* r1 = frame + ((long long)(cp.i + y1) * cp.W + cp.j) * 3;
     float v[3];
-#pragma unroll
-    for (int c = 0; c < 3; ++c) {
-      const float p00 = float(r0[x0 * 3 + c]), p01 = float(r0[x1 * 3 + c]);
-      const float p10 = float(r1[x0 * 3 + c]), p11 = float(r1[x1 * 3 + c]);
-      v[c] = hy * (hx * p00 + lx * p01) + ly * (hx * p10 + lx * p11);
-    }
+    crop_bilinear3(frame, cp.W, cp.i, cp.j, cp.h, cp.w, sh, sw, y, x, v);
     normalise_store(ob + idx, (long long)T * plane, v, mean255, std255);   // sub_ then div_, as the reference
   }
 }

@@ -117,14 +117,9 @@ class _CollatorBase(object):
     @staticmethod
     def _collate(batch):
         """default_collate, except that ClipTickets (uint8 frames + crop/flip decisions on their way to the GPU input
-        kernel, jepa_b200/transforms.py) are kept as per-clip lists: [[ticket_b for b in batch] for each clip]."""
-        first = batch[0]
-        if isinstance(first, (list, tuple)) and len(first) > 0 and isinstance(first[0], (list, tuple)) and \
-                len(first[0]) > 0 and type(first[0][0]).__name__ == "ClipTicket":
-            clips = [[item[0][c] for item in batch] for c in range(len(first[0]))]
-            rest = torch.utils.data.default_collate([tuple(item[1:]) for item in batch])
-            return [clips] + list(rest)
-        return torch.utils.data.default_collate(batch)
+        kernels, jepa_b200/transforms.py) are kept as per-clip lists: [[ticket_b for b in batch] for each clip]."""
+        from .transforms import collate_tickets
+        return collate_tickets(batch)
 
     def __call__(self, batch):
         collated = self._collate(batch)

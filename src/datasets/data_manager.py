@@ -139,12 +139,12 @@ def _eval_dataset(kind, length, transform, clip_len, crop_size, num_clips, num_c
                                       "provided; ImageFolder / ImageNet decoding is outside this package's scope")
         return SyntheticImageDataset(length, crop_size, num_classes, seed=seed)
     if kind == 'synthetic_uint8':
-        from jepa_b200.transforms import GpuEvalVideoTransform
-        if training or not isinstance(transform, GpuEvalVideoTransform):
+        from jepa_b200.transforms import GpuEvalVideoTransform, GpuVideoTransform
+        if not isinstance(transform, GpuVideoTransform if training else GpuEvalVideoTransform):
             raise NotImplementedError(
                 "dataset_type synthetic_uint8 in the frozen evaluation: the training transform uses RandAugment "
-                "(auto_augment) and random erasing (reprob), which have no GPU implementation here; train on "
-                "dataset_type synthetic (pre-normalised clips) - uint8 frames feed validation through vj_clip_views")
+                "(auto_augment) and random erasing (reprob), which run on the GPU only with gpu_augment: true under "
+                "data:; or train on dataset_type synthetic (pre-normalised clips)")
         hw = (int(crop_size * 8 / 7) // 2 * 2, int(crop_size * 4 / 3) // 2 * 2)
         return SyntheticUint8EvalVideoDataset(length, clip_len, hw, transform, num_classes, num_segments=num_clips,
                                               seed=seed)
@@ -168,6 +168,9 @@ def init_data(batch_size, transform=None, shared_transform=None, data='ImageNet'
         dataset = _eval_dataset(kind, length, transform, clip_len, crop_size, num_clips, num_classes, num_views_per_clip,
                                 images, training, seed=rank + (0 if training else 7))
         sampler = DistributedSampler(dataset, num_replicas=world_size, rank=rank, shuffle=training)
+        if collator is None and kind == 'synthetic_uint8' and training:
+            from jepa_b200.transforms import collate_tickets
+            collator = collate_tickets      # [[ticket for each clip] for each segment], labels, indices
         loader = DataLoader(dataset, collate_fn=collator, sampler=sampler, batch_size=batch_size, drop_last=drop_last,
                             pin_memory=pin_mem and kind == 'synthetic', num_workers=num_workers,
                             persistent_workers=num_workers > 0)

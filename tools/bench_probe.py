@@ -3,6 +3,10 @@
 
     python tools/bench_probe.py [--steps K] [--warmup W] [--batch B] [--mode train|val]
 
+--uint8 (train mode) starts each step from B x 8 uint8 clips [16, 256, 340, 3] on the host: the evaluation's training
+transform draws its decisions there (RandAugment, crop, erase), then augment_batch runs them on the GPU; it reports the
+augmentation's time and bytes, and, when oracle/_ref holds the reference, the reference's CPU transform per clip.
+
 --mode val times the validation branch of the same loop (configs/evals/vitl16_k400_16x8x3.yaml: 8 segments x 3 spatial
 views): B clips of uint8 frames [16, 256, 340, 3] per segment on the host -> vj_clip_views (EvalVideoTransform on the GPU,
 one H2D copy of uint8) -> frozen encoder over all 24 views -> 3 classifier calls (attend_across_segments) -> softmax
@@ -52,12 +56,30 @@ def run(args):
     scaler = FlatGradScaler()
     crit = torch.nn.CrossEntropyLoss()
     g = torch.Generator(device="cpu").manual_seed(0)
-    clips = [[torch.randn(B, 3, frames, crop, crop, generator=g).to(device)] for _ in range(n_seg)]
     labels = torch.randint(0, n_cls, (B,), generator=g).to(device)
-    ev = [torch.cuda.Event(enable_timing=True) for _ in range(3)]
-    enc_ms, probe_ms = [], []
+    clips = None
+    ev = [torch.cuda.Event(enable_timing=True) for _ in range(4)]
+    enc_ms, probe_ms, aug_ms, aug_bytes = [], [], [], []
+    if args.uint8:          # the evaluation's training transform (RandAugment + erasing) on the GPU, from uint8 frames
+        from jepa_b200.transforms import augment_batch, make_eval_transforms, pack_augment
+        H0, W0 = 256, 340
+        tf = make_eval_transforms(training=True, random_horizontal_flip=False, random_resize_aspect_ratio=(0.75, 4 / 3),
+                                  random_resize_scale=(0.08, 1.0), reprob=0.25, auto_augment=True, crop_size=crop,
+                                  gpu_augment=True)
+        host = [torch.randint(0, 256, (frames, H0, W0, 3), dtype=torch.uint8, generator=g).numpy()
+                for _ in range(n_seg * B)]
+    else:
+        clips = [[torch.randn(B, 3, frames, crop, crop, generator=g).to(device)] for _ in range(n_seg)]
 
     def step(timed):
+        nonlocal clips
+        if args.uint8:
+            tickets = [tf(x) for x in host]              # host decisions, segment-major
+            ev[3].record()
+            out = augment_batch(tickets, device, crop)
+            clips = [[out[s * B:(s + 1) * B]] for s in range(n_seg)]
+            if timed:
+                aug_bytes.append(_augment_bytes(tickets, pack_augment, out))
         if timed:
             ev[0].record()
         with torch.no_grad():
@@ -84,8 +106,21 @@ def run(args):
         torch.cuda.synchronize()
         enc_ms.append(ev[0].elapsed_time(ev[1]))
         probe_ms.append(ev[1].elapsed_time(ev[2]))
+        if args.uint8:
+            aug_ms.append(ev[3].elapsed_time(ev[0]))
     wall = time.perf_counter() - t0
     clocks = sampler.stop()
+    extra = {}
+    if args.uint8:
+        ms = sorted(aug_ms)[len(aug_ms) // 2]
+        nbytes = sorted(aug_bytes)[len(aug_bytes) // 2]
+        extra = {"data": "synthetic uint8 16x256x340 frames, RandAugment rand-m7-n4-mstd0.5-inc1 + erasing 0.25 on the GPU",
+                 "augment_ms": round(ms, 3), "augment_bytes": nbytes,
+                 "augment_gbps": round(nbytes / (ms * 1e-3) / 1e9, 1),
+                 "augment_timing": "CUDA events from before augment_batch (host packing, uint8 H2D copy, kernels) to "
+                                   "the encoder; bytes from the decision tables (each applied op reads and writes its "
+                                   "clip, a histogram pass reads it, the last pass reads the clip and writes the output)",
+                 "reference_cpu_ms_per_clip": _reference_cpu_ms(host[0], crop)}
     try:
         card = subprocess.run(["nvidia-smi", "--id=0", "--query-gpu=name,power.limit", "--format=csv,noheader,nounits"],
                               capture_output=True, text=True, timeout=30).stdout.strip().split(", ")
@@ -105,7 +140,42 @@ def run(args):
         "gpu": card[0] if card else None,
         "power_limit_w": float(card[1]) if len(card) > 1 else None,
         "clocks": clocks,
+        **extra,
     }), flush=True)
+
+
+def _augment_bytes(tickets, pack_augment, out):
+    import numpy as np
+    from jepa_b200.transforms import AUG_OP
+    buf, frame_bytes, L, flags = pack_augment(tickets)
+    ops = np.frombuffer(buf[frame_bytes + 64 * len(tickets):].numpy().tobytes(), AUG_OP).reshape(L, len(tickets))
+    size = np.array([t.frames.numel() for t in tickets])
+    hist = np.isin(ops["code"], (0, 1, 8))
+    return int((2 * size * (ops["code"] >= 0)).sum() + (size * hist).sum() + size.sum() + out.numel() * out.element_size())
+
+
+def _reference_cpu_ms(clip, crop):
+    """The reference's pre-training transform with RandAugment and erasing (app/vjepa/transforms.py, the same ops as the
+    evaluation's) on one uint8 clip, on this host's CPU, one thread: median ms over 8 calls; None without oracle/_ref."""
+    ref = os.path.join(ROOT, "oracle", "_ref")
+    if not os.path.isdir(os.path.join(ref, "app")):
+        return None
+    code = ("import sys, time, random, numpy as np, torch; sys.path.insert(0, %r); torch.set_num_threads(1)\n"
+            "from app.vjepa.transforms import VideoTransform\n"
+            "tf = VideoTransform(random_resize_scale=(0.08, 1.0), reprob=0.25, auto_augment=True, crop_size=%d)\n"
+            "x = np.load(sys.argv[1]); random.seed(0); np.random.seed(0); torch.manual_seed(0); ts = []\n"
+            "for _ in range(8):\n    t0 = time.perf_counter(); tf(x); ts.append(time.perf_counter() - t0)\n"
+            "print(sorted(ts)[4] * 1e3)") % (ref, crop)
+    import tempfile
+    import numpy as np
+    with tempfile.TemporaryDirectory() as d:
+        path = os.path.join(d, "clip.npy")
+        np.save(path, clip)
+        r = subprocess.run([sys.executable, "-c", code, path], capture_output=True, text=True, cwd=d, timeout=600)
+    try:
+        return round(float(r.stdout.strip().splitlines()[-1]), 1)
+    except (ValueError, IndexError):
+        return None
 
 
 def _card():
@@ -213,6 +283,8 @@ def main():
     ap.add_argument("--batch", type=int, default=4, help="clips per step (K400 eval config: 4 per GPU)")
     ap.add_argument("--mode", choices=("train", "val"), default="train",
                     help="train: probe training step; val: validation step from uint8 frames")
+    ap.add_argument("--uint8", action="store_true",
+                    help="train mode: uint8 frames through the GPU training transform (RandAugment, erasing)")
     args = ap.parse_args()
     run(args) if args.mode == "train" else run_val(args)
 
