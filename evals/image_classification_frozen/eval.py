@@ -173,7 +173,11 @@ def run_one_epoch(device, training, encoder, classifier, scaler, optimizer, sche
             wd_scheduler.step()
 
         # (no autocast: the kernels compute bf16 x bf16 -> fp32 regardless; see the module docstring)
-        imgs, labels = data[0].to(device), data[1].to(device)
+        if isinstance(data[0], list):       # uint8 image tickets: the transform's pixel work runs on the GPU
+            imgs = data_loader.dataset.transform.batch(data[0], device)
+        else:
+            imgs = data[0].to(device)
+        labels = data[1].to(device)
         with torch.no_grad():
             outputs = encoder(imgs)
             if not training:
@@ -208,13 +212,27 @@ def run_one_epoch(device, training, encoder, classifier, scaler, optimizer, sche
 
 def make_dataloader(dataset_name, root_path, image_folder, batch_size, world_size, rank, resolution=224, training=False,
                     subset_file=None, num_classes=None, synthetic_length=None):
-    """eval.py:379-423.  The reference's image transforms (timm RandAugment + random erasing for training, PIL resize +
-    centre crop for validation) are CPU pipelines outside this package; the synthetic dataset yields pre-normalised
-    [3, S, S] images and needs none, and other datasets raise in init_data."""
-    data_loader, _ = init_data(data=dataset_name, transform=None, batch_size=batch_size, world_size=world_size, rank=rank,
-                               root_path=root_path, image_folder=image_folder, training=training, copy_data=False,
-                               drop_last=False, subset_file=subset_file, crop_size=resolution, num_workers=0,
-                               num_classes=num_classes, images=True, synthetic_length=synthetic_length)
+    """eval.py:379-423.  ImageNet / iNat21 / Places205 (ImageFolder trees) and synthetic_uint8 images get the reference's
+    transforms with the pixel work on the GPU (jepa_b200/image_transforms.py): timm's AutoAugment 'original' + random
+    erasing for training, Resize + CenterCrop for validation, both bit-exact; the loader yields uint8 image tickets and
+    run_one_epoch makes [B, 3, S, S] on the device.  The synthetic dataset yields pre-normalised images and needs none."""
+    from jepa_b200.image_transforms import GpuImageEvalTransform, GpuImageTransform
+    normalization = ((0.485, 0.456, 0.406), (0.229, 0.224, 0.225))
+    kind = str(dataset_name).lower()
+    transform, num_workers = None, 0
+    if kind != 'synthetic':
+        if training:
+            logger.info('implementing auto-agument strategy')
+            transform = GpuImageTransform(crop_size=resolution, normalize=normalization, re_prob=0.25)
+        else:
+            transform = GpuImageEvalTransform(crop_size=resolution, normalize=normalization)
+        if kind != 'synthetic_uint8':
+            num_workers = 8                 # PIL decoding in loader workers, as the reference's init_data default
+    data_loader, _ = init_data(data=dataset_name, transform=transform, batch_size=batch_size, world_size=world_size,
+                               rank=rank, root_path=root_path, image_folder=image_folder, training=training,
+                               copy_data=False, drop_last=False, subset_file=subset_file, crop_size=resolution,
+                               num_workers=num_workers, num_classes=num_classes, images=True,
+                               synthetic_length=synthetic_length)
     return data_loader
 
 

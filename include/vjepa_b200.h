@@ -248,6 +248,32 @@ int vj_clip_augment(void* buf0, void* buf1, const void* clips, const void* ops, 
                     int n_layers, void* out, int out_f32, int B, int T, int S, const float* mean3, const float* std3,
                     void* stream);
 
+/* Frozen image evaluation, validation: uint8 RGB images of mixed sizes -> PIL 12's Image.resize (BILINEAR / BICUBIC,
+ * Resample.c 8-bit fixed point, bit-exact) -> S x S window -> torchvision ToTensor + Normalize in fp32 ((v / 255 - mean) /
+ * std, each step rounded) -> out [B, 3, S, S] fp32 or bf16.  2 launches.  src_u8: device buffer of every image [H, W, 3];
+ * jobs: device table, one 64-byte record per image = {int64 byte offset of the image in src_u8, int64 byte offset of its
+ * rows in tmp, int32 W, first source row r0, row count nrows, first source column c0, xtab, ytab, xk, yk, flip, pad[3]};
+ * coefs: device int32 table; S entries of xk ints from xtab (output columns) and S entries of yk ints from ytab (output
+ * rows), each {first tap (columns: from c0; rows: from r0), tap count, int32 weights at 22 fractional bits}.  tmp: device
+ * uint8 scratch of nrows * S * 3 bytes per image at its tmp offset.  mean3 / std3: HOST arrays of 3 floats.  Replaces
+ * Resize(int(S * 256 / 224)) / CenterCrop(S) / ToTensor / Normalize of evals/image_classification_frozen/eval.py:405-409;
+ * the tables come from jepa_b200/image_transforms.py. */
+int vj_image_views(const void* src_u8, const void* jobs, const void* coefs, void* tmp, void* out, int out_f32, int B, int S,
+                   const float* mean3, const float* std3, void* stream);
+
+/* Frozen image evaluation, training: the resample of vj_image_views over each image's random-resized-crop box (jobs /
+ * coefs / tmp as there; flip mirrors the result) into buf0 [B, S, S, 3] -> n_layers AutoAugment layers through the
+ * RandAugment kernels of vj_clip_augment (T = 1, clips / ops / hist / layer_flags as there; geometric ops fill with the
+ * HOST RGB fill3) -> ToTensor + Normalize (as vj_image_views) -> erase box copied from noise (device fp32; a clip record's
+ * seed field is the element offset of its [3, eh, ew] block; may be NULL when no image erases) -> out [B, 3, S, S] fp32
+ * or bf16.  At most 2 + 2 * n_layers + 1 launches.  Replaces timm's create_transform(is_training=True,
+ * auto_augment='original', interpolation='bicubic', re_prob=0.25, re_mode='pixel', re_count=1) of
+ * evals/image_classification_frozen/eval.py:392-403; the decisions come from jepa_b200/image_transforms.py. */
+int vj_image_augment(const void* src_u8, const void* jobs, const void* coefs, void* tmp, void* buf0, void* buf1,
+                     const void* clips, const void* ops, void* hist, const int* layer_flags, int n_layers,
+                     const float* noise, void* out, int out_f32, int B, int S, const float* mean3, const float* std3,
+                     const unsigned char* fill3, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -21,6 +21,8 @@ SIGNATURES = {
     "vj_clip_preprocess": (I, [P, P, P, I, I, I, I, P, P, P]),
     "vj_clip_views": (I, [P, P, P, P, I, I, I, I, P, P, P]),
     "vj_clip_augment": (I, [P, P, P, P, P, P, I, P, I, I, I, I, P, P, P]),
+    "vj_image_views": (I, [P, P, P, P, P, I, I, I, P, P, P]),
+    "vj_image_augment": (I, [P, P, P, P, P, P, P, P, P, P, I, P, P, I, I, I, P, P, P, P]),
     "vj_gemm": (I, [P, L, I, P, L, I, P, L, I, I, I, I, P, F, I, P, L, I, P, I, P, L, I, I, P]),
     "vj_attn_fwd": (I, [P, P, P, P, I, I, I, I, I, F, P]),
     "vj_attn_bwd": (I, [P, P, P, P, P, P, P, P, I, I, I, I, I, F, P]),

@@ -19,7 +19,8 @@
 //              Color: L = (19595 R + 38470 G + 7471 B + 0x8000) >> 16; Contrast: int(mean(L) + 0.5) from the L
 //              histogram; Brightness: 0; Sharpness: SMOOTH = (3 x 3 sum with centre weight 5 + 6) // 13, border copied.
 //   Affine     Rotate / Shear / Translate: source = (m0 (x+.5) + m1 (y+.5) + m2, m3 (x+.5) + m4 (y+.5) + m5) in double,
-//              outside the frame: fill 128; else PIL's bicubic (Geometry.c BICUBIC, clamped 4 x 4 taps) in double,
+//              outside the frame: the fill colour (128 for RandAugment, the launch's RGB for AutoAugment); else
+//              PIL's bicubic (Geometry.c BICUBIC, clamped 4 x 4 taps) in double,
 //              clipped and truncated.
 // Every float / double operation that must round as PIL's compiled C does is an explicit _rn intrinsic, so no
 // multiply-add is contracted.
@@ -33,24 +34,6 @@ namespace vj {
 enum RaOp {   // jepa_b200.transforms.RA_OPS
   kAutoContrast, kEqualize, kInvert, kRotate, kPosterize, kSolarize, kSolarizeAdd, kColor, kContrast, kBrightness,
   kSharpness, kShearX, kShearY, kTranslateX, kTranslateY
-};
-
-struct AugClip {            // per clip, 64 bytes
-  long long off;            // byte offset of the clip's frames [T, H, W, 3] in each work buffer
-  int H, W;
-  int i, j, h, w;           // crop box
-  int flip;                 // mirror the output horizontally
-  int final_buf;            // work buffer holding the clip after the last layer (0 or 1)
-  int etop, eleft, eh, ew;  // erase box in output coordinates (after the flip); eh == 0: no erase
-  unsigned long long seed;  // Philox key of the erase noise
-};
-
-struct AugOp {              // per (layer, clip), 64 bytes
-  double m[6];              // inverse affine matrix of the geometric ops
-  int code;                 // RaOp, -1: skipped (the clip stays in in_buf)
-  float fval;               // blend factor
-  int ival;                 // posterize bits / solarize threshold / solarize-add amount
-  int in_buf;               // read from work buffer in_buf, write to 1 - in_buf
 };
 
 constexpr int kBins = 1024;   // R, G, B, L histograms of one frame
@@ -104,7 +87,7 @@ __device__ __forceinline__ uint8_t blend(int d, int v, float a) {   // Image.ble
 
 __global__ void __launch_bounds__(256) ra_apply_kernel(uint8_t* __restrict__ buf0, uint8_t* __restrict__ buf1,
                                                        const AugClip* __restrict__ clips, const AugOp* __restrict__ ops,
-                                                       const int* __restrict__ hist, int T) {
+                                                       const int* __restrict__ hist, int T, uchar3 fill) {
   const int b = blockIdx.z, t = blockIdx.y;
   const AugOp op = ops[b];
   if (op.code < 0) return;
@@ -176,7 +159,7 @@ __global__ void __launch_bounds__(256) ra_apply_kernel(uint8_t* __restrict__ buf
       const double xin = __dadd_rn(__dadd_rn(__dmul_rn(op.m[0], xs), __dmul_rn(op.m[1], ys)), op.m[2]);
       const double yin = __dadd_rn(__dadd_rn(__dmul_rn(op.m[3], xs), __dmul_rn(op.m[4], ys)), op.m[5]);
       if (!(xin >= 0.0 && xin < double(W) && yin >= 0.0 && yin < double(H))) {
-        o[0] = o[1] = o[2] = 128;
+        o[0] = fill.x; o[1] = fill.y; o[2] = fill.z;
         continue;
       }
       const double xi = __dsub_rn(xin, 0.5), yi = __dsub_rn(yin, 0.5);
@@ -284,6 +267,30 @@ __global__ void __launch_bounds__(256) augment_final_kernel(const uint8_t* __res
   }
 }
 
+// The RandAugment / AutoAugment layers of one batch: per layer an optional histogram pass and one apply pass over every
+// (clip, frame), ping-ponging between b0 and b1 as the ops' in_buf fields say.  Shared by vj_clip_augment and
+// vj_image_augment (image.cu); geometric ops fill uncovered pixels with `fill`.
+int ra_layers(uint8_t* b0, uint8_t* b1, const void* clips, const void* ops, void* hist, const int* layer_flags,
+              int n_layers, int B, int T, uchar3 fill, cudaStream_t s) {
+  const auto* cl = reinterpret_cast<const AugClip*>(clips);
+  for (int l = 0; l < n_layers; ++l) {
+    if (!(layer_flags[l] & 1)) continue;                 // every op of this layer skipped
+    const auto* op = reinterpret_cast<const AugOp*>(ops) + (long long)l * B;
+    int* h = reinterpret_cast<int*>(hist) + (long long)l * B * T * kBins;
+    const dim3 grid(32, T, B);
+    if (layer_flags[l] & 2) {                             // some op of this layer reads the frame's histogram
+      VJ_CUDA(cudaMemsetAsync(h, 0, sizeof(int) * (size_t)B * T * kBins, s));
+      ra_hist_kernel<<<grid, 256, 0, s>>>(b0, b1, cl, op, h, T);
+      VJ_CUDA(cudaGetLastError());
+      vj::count_launch(1);
+    }
+    ra_apply_kernel<<<grid, 256, 0, s>>>(b0, b1, cl, op, h, T, fill);
+    VJ_CUDA(cudaGetLastError());
+    vj::count_launch(1);
+  }
+  return 0;
+}
+
 }  // namespace vj
 
 extern "C" int vj_clip_augment(void* buf0, void* buf1, const void* clips, const void* ops, void* hist,
@@ -303,21 +310,8 @@ extern "C" int vj_clip_augment(void* buf0, void* buf1, const void* clips, const 
   auto* b0 = reinterpret_cast<uint8_t*>(buf0);
   auto* b1 = reinterpret_cast<uint8_t*>(buf1);
   const auto* cl = reinterpret_cast<const AugClip*>(clips);
-  for (int l = 0; l < n_layers; ++l) {
-    if (!(layer_flags[l] & 1)) continue;                 // every op of this layer skipped
-    const auto* op = reinterpret_cast<const AugOp*>(ops) + (long long)l * B;
-    int* h = reinterpret_cast<int*>(hist) + (long long)l * B * T * kBins;
-    const dim3 grid(32, T, B);
-    if (layer_flags[l] & 2) {                             // some op of this layer reads the frame's histogram
-      VJ_CUDA(cudaMemsetAsync(h, 0, sizeof(int) * (size_t)B * T * kBins, s));
-      ra_hist_kernel<<<grid, 256, 0, s>>>(b0, b1, cl, op, h, T);
-      VJ_CUDA(cudaGetLastError());
-      vj::count_launch(1);
-    }
-    ra_apply_kernel<<<grid, 256, 0, s>>>(b0, b1, cl, op, h, T);
-    VJ_CUDA(cudaGetLastError());
-    vj::count_launch(1);
-  }
+  if (const int rc = ra_layers(b0, b1, clips, ops, hist, layer_flags, n_layers, B, T, make_uchar3(128, 128, 128), s))
+    return rc;
   const float3 mean255 = make_float3(mean3[0] * 255.f, mean3[1] * 255.f, mean3[2] * 255.f);       // host arrays
   const float3 std255 = make_float3(std3[0] * 255.f, std3[1] * 255.f, std3[2] * 255.f);
   dim3 grid((S * S + 255) / 256, T, B);

@@ -35,4 +35,29 @@ __device__ __forceinline__ void crop_bilinear3(const uint8_t* frame, int W, int 
   }
 }
 
+// Records of vj_clip_augment / vj_image_augment (jepa_b200/transforms.py AUG_CLIP / AUG_OP)
+struct AugClip {            // per clip, 64 bytes
+  long long off;            // byte offset of the clip's frames [T, H, W, 3] in each work buffer
+  int H, W;
+  int i, j, h, w;           // crop box
+  int flip;                 // mirror the output horizontally
+  int final_buf;            // work buffer holding the clip after the last layer (0 or 1)
+  int etop, eleft, eh, ew;  // erase box in output coordinates (after the flip); eh == 0: no erase
+  unsigned long long seed;  // vj_clip_augment: Philox key of the erase noise; vj_image_augment: element offset of
+                            // the host-drawn noise [3, eh, ew] in the noise buffer
+};
+
+struct AugOp {              // per (layer, clip), 64 bytes
+  double m[6];              // inverse affine matrix of the geometric ops
+  int code;                 // RaOp, -1: skipped (the clip stays in in_buf)
+  float fval;               // blend factor
+  int ival;                 // posterize bits / solarize threshold / solarize-add amount
+  int in_buf;               // read from work buffer in_buf, write to 1 - in_buf
+};
+
+// RandAugment / AutoAugment layers over B clips of T frames in the work buffers b0 / b1 (augment.cu; records and tables
+// as documented at vj_clip_augment).  fill: RGB of the pixels a geometric op leaves uncovered.  Returns 0 or an error.
+int ra_layers(uint8_t* b0, uint8_t* b1, const void* clips, const void* ops, void* hist, const int* layer_flags,
+              int n_layers, int B, int T, uchar3 fill, cudaStream_t s);
+
 }  // namespace vj

@@ -5,9 +5,14 @@ Video decoding / augmentation (decord, PIL) is CPU dataloader work outside the a
 metric is defined on (random N(0,1) clips, the distribution of normalised video) behind the same
 `init_data(...) -> (loader, sampler)` contract, so `app.vjepa.train.main` runs end to end.
 """
+import os
+from logging import getLogger
+
 import torch
 from torch.utils.data import DataLoader, Dataset
 from torch.utils.data.distributed import DistributedSampler
+
+logger = getLogger()
 
 
 class SyntheticVideoDataset(Dataset):
@@ -130,13 +135,67 @@ class SyntheticImageDataset(Dataset):
         return self._patterns[label] + self.noise * torch.randn(self._patterns[label].shape, generator=g), label
 
 
+class SyntheticUint8ImageDataset(Dataset):
+    """Decoded-image stand-in for the frozen image evaluation: (transform(uint8 [H, W, 3]), label) with a size that varies
+    per item (landscape and portrait, like decoded photos), class pattern + noise clamped to 0..255, label
+    index % num_classes.  The class pattern is a dark / bright texture whose orientation (label % 3: horizontal stripes,
+    vertical stripes, checkerboard) and period (16 + 4 * (label // 3) pixels) survive what the training transform does
+    to an image: crops down to 8 % of the area, flips, rotations up to 27 degrees, colour and histogram ops, inversion,
+    erasing, and Solarize at any of its thresholds (dark 40 and bright 140 stay apart after 255 - v).  With the GPU image transforms the items are tickets and the pixel work runs on the GPU."""
+    SIZES = ((3, 4), (4, 3), (9, 16), (1, 1), (5, 4), (3, 5))     # height : width
+
+    def __init__(self, length, crop_size, num_classes, transform, seed=0):
+        self.length, self.crop_size, self.num_classes, self.transform = length, crop_size, num_classes, transform
+        self.seed = seed
+
+    def __len__(self):
+        return self.length
+
+    def __getitem__(self, index):
+        g = torch.Generator().manual_seed(self.seed * 1000003 + index)
+        label = index % self.num_classes
+        short = int(self.crop_size * (1.0 + 0.5 * torch.rand(1, generator=g).item()))
+        a, b = self.SIZES[index % len(self.SIZES)]
+        H, W = (short * a // min(a, b), short * b // min(a, b))
+        half = 8 + 2 * (label // 3)
+        y, x = torch.meshgrid(torch.arange(H) // half, torch.arange(W) // half, indexing='ij')
+        bright = (y, x, y + x)[label % 3] % 2
+        base = 40. + 100. * bright[..., None].float() + _class_pattern(label, (3,), 8.)
+        img = (base + 8. * torch.randn(base.shape, generator=g)).round_().clamp_(0, 255).to(torch.uint8).numpy()
+        return (self.transform(img) if self.transform is not None else torch.from_numpy(img)), label
+
+
+IMAGE_FOLDERS = ('imagenet', 'inat21', 'places205')
+
+
+def _image_folder_loader(transform, batch_size, collator, pin_mem, num_workers, world_size, rank, root_path,
+                         image_folder, training, drop_last, persistent_workers):
+    """src/datasets/image_dataset.py of the reference: torchvision ImageFolder at root_path/image_folder/{train,val}/
+    (default PIL loader, RGB), DistributedSampler(dataset, world_size, rank) (shuffled on both splits)."""
+    import torchvision
+    from jepa_b200.image_transforms import GpuImageEvalTransform, collate_image_tickets
+    data_path = os.path.join(root_path, image_folder, 'train/' if training else 'val/')
+    logger.info(f'data-path {data_path}')
+    dataset = torchvision.datasets.ImageFolder(root=data_path, transform=transform)
+    sampler = DistributedSampler(dataset=dataset, num_replicas=world_size, rank=rank)
+    tickets = isinstance(transform, GpuImageEvalTransform)
+    if collator is None and tickets:
+        collator = collate_image_tickets        # [tickets], labels: the pixels are made on the GPU
+    loader = DataLoader(dataset, collate_fn=collator, sampler=sampler, batch_size=batch_size, drop_last=drop_last,
+                        pin_memory=pin_mem and not tickets, num_workers=num_workers,
+                        persistent_workers=persistent_workers and num_workers > 0)
+    return loader, sampler
+
+
 def _eval_dataset(kind, length, transform, clip_len, crop_size, num_clips, num_classes, num_views_per_clip, images,
                   training, seed):
     """The frozen evaluations' synthetic datasets (opt-in through num_classes)."""
     if images:
+        if kind == 'synthetic_uint8':
+            return SyntheticUint8ImageDataset(length, crop_size, num_classes, transform, seed=seed)
         if kind != 'synthetic':
-            raise NotImplementedError(f"image evaluation dataset {kind!r}: only 'synthetic' (pre-normalised images) is "
-                                      "provided; ImageFolder / ImageNet decoding is outside this package's scope")
+            raise NotImplementedError(f"image evaluation dataset {kind!r}: 'synthetic', 'synthetic_uint8' and the "
+                                      f"ImageFolder datasets {IMAGE_FOLDERS} are provided")
         return SyntheticImageDataset(length, crop_size, num_classes, seed=seed)
     if kind == 'synthetic_uint8':
         from jepa_b200.transforms import GpuEvalVideoTransform, GpuVideoTransform
@@ -160,15 +219,25 @@ def init_data(batch_size, transform=None, shared_transform=None, data='ImageNet'
               repeat_wds=False, ipe=300, log_dir=None, crop_size=224, synthetic_length=None, num_classes=None,
               num_views_per_clip=None, images=False):
     """num_classes (opt-in): the frozen evaluations' labelled synthetic items (SyntheticEvalVideoDataset /
-    SyntheticUint8EvalVideoDataset with num_views_per_clip views per segment, SyntheticImageDataset with images=True);
-    left at None, the pre-training items are unchanged."""
+    SyntheticUint8EvalVideoDataset with num_views_per_clip views per segment, SyntheticImageDataset /
+    SyntheticUint8ImageDataset with images=True); left at None, the pre-training items are unchanged.  With images=True,
+    data ImageNet / iNat21 / Places205 (any case) is an ImageFolder at root_path/image_folder/{train,val}/."""
     kind = str(data).lower()
+    if images and kind in IMAGE_FOLDERS:
+        if subset_file is not None or copy_data:
+            raise NotImplementedError("ImageFolder datasets: subset_file and copy_data are not supported; point "
+                                      "root_path / image_folder at the images to use")
+        return _image_folder_loader(transform, batch_size, collator, pin_mem, num_workers, world_size, rank, root_path,
+                                    image_folder, training, drop_last, persistent_workers)
     if num_classes is not None:
         length = synthetic_length or batch_size * world_size * ipe
         dataset = _eval_dataset(kind, length, transform, clip_len, crop_size, num_clips, num_classes, num_views_per_clip,
                                 images, training, seed=rank + (0 if training else 7))
         sampler = DistributedSampler(dataset, num_replicas=world_size, rank=rank, shuffle=training)
-        if collator is None and kind == 'synthetic_uint8' and training:
+        if collator is None and kind == 'synthetic_uint8' and images:
+            from jepa_b200.image_transforms import collate_image_tickets
+            collator = collate_image_tickets    # [tickets], labels
+        elif collator is None and kind == 'synthetic_uint8' and training:
             from jepa_b200.transforms import collate_tickets
             collator = collate_tickets      # [[ticket for each clip] for each segment], labels, indices
         loader = DataLoader(dataset, collate_fn=collator, sampler=sampler, batch_size=batch_size, drop_last=drop_last,

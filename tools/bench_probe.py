@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Frozen-evaluation probe training step (or validation step), clips/sec, at the ViT-L/16 K400 shape.
 
-    python tools/bench_probe.py [--steps K] [--warmup W] [--batch B] [--mode train|val]
+    python tools/bench_probe.py [--steps K] [--warmup W] [--batch B] [--mode train|val|image]
 
 --uint8 (train mode) starts each step from B x 8 uint8 clips [16, 256, 340, 3] on the host: the evaluation's training
 transform draws its decisions there (RandAugment, crop, erase), then augment_batch runs them on the GPU; it reports the
@@ -12,6 +12,14 @@ views): B clips of uint8 frames [16, 256, 340, 3] per segment on the host -> vj_
 one H2D copy of uint8) -> frozen encoder over all 24 views -> 3 classifier calls (attend_across_segments) -> softmax
 average.  It also times vj_clip_views alone on device-resident frames and reports GB/s (uint8 read + output written,
 from the shapes).
+
+--mode image times the frozen IMAGE evaluation's probe training step at the ViT-L/16 in1k shape
+(configs/evals/vitl16_in1k.yaml: 16 frames, each image repeated over them as the evaluation's forward pre-hook does,
+batch 16, 1000 classes).  With --uint8 each step starts from B uint8 500x375 images on the host: GpuImageTransform draws
+the decisions (crop, flip, AutoAugment 'original', erasing) and vj_image_augment makes [B, 3, 224, 224] on the GPU;
+without it the images are pre-normalised and device-resident.  It also reports vj_image_augment and vj_image_views alone
+(CUDA events, staged buffers already on the device) and, when oracle/_ref holds the reference, the reference's CPU
+training transform per image (timm's composition of its pieces, one thread).
 
 One step is the training branch of the reference's evaluation loop (evals/video_classification_frozen/eval.py:317-373
 with configs/evals/vitl16_k400_16x8x3.yaml): B clips of 8 segments x 16 frames at 224^2 through the frozen encoder under
@@ -276,16 +284,177 @@ def run_val(args):
     }), flush=True)
 
 
+def run_image(args):
+    import numpy as np
+    from jepa_b200 import image_transforms as it
+    from jepa_b200.models import vit_large
+    from jepa_b200.optim import FlatAdamW, FlatGradScaler
+    from jepa_b200.pooler import AttentiveClassifier
+    from jepa_b200.step import clip_grad_norm_
+    device = torch.device("cuda:0")
+    torch.manual_seed(0)
+    B = args.batch or 16
+    frames, crop, n_cls, H0, W0 = 16, 224, 1000, 375, 500
+    enc = vit_large(img_size=crop, num_frames=frames, tubelet_size=2, uniform_power=True).to(device).eval()
+    for p in enc.parameters():
+        p.requires_grad = False
+    clf = AttentiveClassifier(embed_dim=enc.embed_dim, num_heads=enc.num_heads, depth=1, num_classes=n_cls).to(device)
+    groups = [{"params": [p for n, p in clf.named_parameters() if ("bias" not in n) and (len(p.shape) != 1)]},
+              {"params": [p for n, p in clf.named_parameters() if ("bias" in n) or (len(p.shape) == 1)],
+               "WD_exclude": True, "weight_decay": 0}]
+    opt = FlatAdamW(groups, lr=1e-3, weight_decay=0.01)
+    scaler = FlatGradScaler()
+    crit = torch.nn.CrossEntropyLoss()
+    g = torch.Generator(device="cpu").manual_seed(0)
+    labels = torch.randint(0, n_cls, (B,), generator=g).to(device)
+    tf = it.GpuImageTransform(crop_size=crop)
+    host = [torch.randint(0, 256, (H0, W0, 3), dtype=torch.uint8, generator=g).numpy() for _ in range(B)]
+    imgs = None if args.uint8 else torch.randn(B, 3, crop, crop, generator=g).to(device)
+    ev = [torch.cuda.Event(enable_timing=True) for _ in range(4)]
+    enc_ms, probe_ms, tf_ms, host_ms = [], [], [], []
+
+    def step(timed):
+        nonlocal imgs
+        if args.uint8:
+            t0 = time.perf_counter()
+            tickets = [tf(x) for x in host]            # host decisions (what the loader workers do)
+            if timed:
+                host_ms.append((time.perf_counter() - t0) * 1e3)
+            ev[3].record()
+            imgs = tf.batch(tickets, device)
+        if timed:
+            ev[0].record()
+        with torch.no_grad():
+            outputs = enc(imgs.unsqueeze(2).repeat(1, 1, frames, 1, 1))
+        if timed:
+            ev[1].record()
+        loss = crit(clf(outputs), labels)
+        scaler.scale(loss).backward()
+        scaler.unscale_(opt)
+        clip_grad_norm_(clf, 1.0)
+        scaler.step(opt)
+        scaler.update()
+        opt.zero_grad()
+        if timed:
+            ev[2].record()
+
+    for _ in range(args.warmup):
+        step(False)
+    torch.cuda.synchronize()
+    sampler = ClockSampler(0)
+    t0 = time.perf_counter()
+    for _ in range(args.steps):
+        step(True)
+        torch.cuda.synchronize()
+        enc_ms.append(ev[0].elapsed_time(ev[1]))
+        probe_ms.append(ev[1].elapsed_time(ev[2]))
+        if args.uint8:
+            tf_ms.append(ev[3].elapsed_time(ev[0]))
+    wall = time.perf_counter() - t0
+    clocks = sampler.stop()
+
+    # the kernels alone, on staged batches already on the device
+    images = [torch.from_numpy(x) for x in host]
+    tickets = [tf(x) for x in host]
+    packed = it.pack_image_augment(images, [(t.box, (crop, crop), (0, 0), True, t.flip) for t in tickets], crop,
+                                   [t.ops for t in tickets], [t.erase for t in tickets], [t.noise for t in tickets])
+    dev, _ = it.to_device(packed["pk"], device)
+    scratch = it.image_augment_scratch(packed, device)
+    out = torch.empty(B, 3, crop, crop, device=device)
+    fill = it.fill_color(it.DEFAULT_NORMALIZE[0])
+    vpk, jobs_off, coefs_off, tmp_bytes = it.pack_image_views(images, crop)
+    vdev, _ = it.to_device(vpk, device)
+    vtmp = torch.empty(max(tmp_bytes, 16), dtype=torch.uint8, device=device)
+    aug_k, views_k = [], []
+    for i in range(args.warmup + args.steps):
+        ev[0].record()
+        it.launch_image_augment(dev, packed, scratch, out, *it.DEFAULT_NORMALIZE, fill)
+        ev[1].record()
+        it.launch_image_views(vdev, jobs_off, coefs_off, vtmp, out, *it.DEFAULT_NORMALIZE)
+        ev[2].record()
+        torch.cuda.synchronize()
+        if i >= args.warmup:
+            aug_k.append(ev[0].elapsed_time(ev[1]))
+            views_k.append(ev[1].elapsed_time(ev[2]))
+    card = _card()
+    med = lambda v: round(sorted(v)[len(v) // 2], 3) if v else None
+    print(json.dumps({
+        "metric": "images/sec ViT-L/16 in1k frozen-evaluation probe training step (16x224^2 per image, 1000 classes)",
+        "value": round(B * args.steps / wall, 2), "unit": "images/s", "n_gpus": 1, "steps": args.steps,
+        "warmup": args.warmup, "higher_is_better": True, "dtype": "bf16",
+        "data": (f"uint8 {W0}x{H0} images on the host, timm AutoAugment 'original' + erasing 0.25 on the GPU"
+                 if args.uint8 else "pre-normalised images resident on the device"),
+        "config": {"workload": f"batch {B}/GPU, each image repeated over {frames} frames ({enc.num_patches} tokens), "
+                               "AttentiveClassifier depth 1, CrossEntropyLoss, FlatGradScaler + clip 1.0 + FlatAdamW"},
+        "encoder_fwd_ms": med(enc_ms),
+        "probe_fwd_bwd_opt_ms": med(probe_ms),
+        "transform_ms": med(tf_ms),
+        "host_decisions_ms": med(host_ms),
+        "image_augment_kernels_ms": med(aug_k),
+        "image_views_kernels_ms": med(views_k),
+        "timing": "CUDA events per step, median over the timed steps; value = wall clock over the timed steps; "
+                  "transform_ms: from before the batch call (host packing, one uint8 H2D copy, kernels) to the encoder; "
+                  "host_decisions_ms: the transform's __call__ for the whole batch on one thread; *_kernels_ms: "
+                  f"one launch sequence for {B} images staged on the device",
+        "reference_cpu_ms_per_image": _reference_image_cpu_ms(host[0], crop),
+        "gpu": card[0] if card else None,
+        "power_limit_w": float(card[1]) if len(card) > 1 else None,
+        "clocks": clocks,
+    }), flush=True)
+
+
+def _reference_image_cpu_ms(img, crop):
+    """The reference's image training transform (timm's create_transform composition of the reference's
+    RandomResizedCropAndInterpolation, RandomHorizontalFlip, AutoAugment of its AugmentOp, ToTensor, Normalize and
+    RandomErasing) on one uint8 image, on this host's CPU, one thread: median ms over 16 calls; None without oracle/_ref."""
+    ref = os.path.join(ROOT, "oracle", "_ref")
+    if not os.path.isdir(os.path.join(ref, "src")):
+        return None
+    from jepa_b200.image_transforms import AA_POLICY, DEFAULT_NORMALIZE, fill_color
+    code = ("import sys, time, random, numpy as np, torch; sys.path.insert(0, %r)\n"
+            "torch.set_num_threads(1)\n"
+            "from PIL import Image; from torchvision import transforms as T\n"
+            "import src.datasets.utils.video.randaugment as ra, src.datasets.utils.video.randerase as rr\n"
+            "from src.datasets.utils.video.transforms import RandomResizedCropAndInterpolation\n"
+            "AA_POLICY, fill, N, S = %r, %r, %r, %d\n"
+            "hp = dict(translate_const=int(S * 0.45), img_mean=fill, interpolation=Image.BICUBIC)\n"
+            "pol = [[ra.AugmentOp(n, prob=p, magnitude=m or 0, hparams=hp) for n, p, m in sp] for sp in AA_POLICY]\n"
+            "pre = T.Compose([RandomResizedCropAndInterpolation(S, interpolation='bicubic'), T.RandomHorizontalFlip()])\n"
+            "post = T.Compose([T.ToTensor(), T.Normalize(*N)])\n"
+            "er = rr.RandomErasing(0.25, mode='pixel', max_count=1, device='cpu')\n"
+            "x = Image.fromarray(np.load(sys.argv[1])); random.seed(0); torch.manual_seed(0); ts = []\n"
+            "for _ in range(16):\n"
+            "    t0 = time.perf_counter(); y = pre(x)\n"
+            "    for op in random.choice(pol): y = op(y)\n"
+            "    er(post(y)); ts.append(time.perf_counter() - t0)\n"
+            "print(sorted(ts)[8] * 1e3)") % (ref, AA_POLICY, fill_color(DEFAULT_NORMALIZE[0]), DEFAULT_NORMALIZE, crop)
+    import tempfile
+    import numpy as np
+    with tempfile.TemporaryDirectory() as d:
+        path = os.path.join(d, "img.npy")
+        np.save(path, img)
+        r = subprocess.run([sys.executable, "-c", code, path], capture_output=True, text=True, cwd=d, timeout=600)
+    try:
+        return round(float(r.stdout.strip().splitlines()[-1]), 2)
+    except (ValueError, IndexError):
+        return None
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--steps", type=int, default=10)
     ap.add_argument("--warmup", type=int, default=3)
-    ap.add_argument("--batch", type=int, default=4, help="clips per step (K400 eval config: 4 per GPU)")
-    ap.add_argument("--mode", choices=("train", "val"), default="train",
-                    help="train: probe training step; val: validation step from uint8 frames")
+    ap.add_argument("--batch", type=int, default=None,
+                    help="clips (images) per step; default 4 (K400 eval config) or, in image mode, 16 (in1k config)")
+    ap.add_argument("--mode", choices=("train", "val", "image"), default="train",
+                    help="train: probe training step; val: validation step from uint8 frames; image: image probe step")
     ap.add_argument("--uint8", action="store_true",
-                    help="train mode: uint8 frames through the GPU training transform (RandAugment, erasing)")
+                    help="train / image mode: uint8 frames / images through the GPU training transform")
     args = ap.parse_args()
+    if args.mode == "image":
+        run_image(args)
+        return
+    args.batch = args.batch or 4
     run(args) if args.mode == "train" else run_val(args)
 
 
