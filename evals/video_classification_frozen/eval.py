@@ -3,6 +3,7 @@
 Same config keys, log lines, CSV columns and checkpoint dictionary as the reference (evals/video_classification_frozen/
 eval.py:67-561), with every step on the sm_90a kernels of jepa_b200:
   frozen encoder, all clips and views in one batch -> ClipAggregation (jepa_b200.pooler)
+  image encoder (pretrain frames_per_clip == 1)     -> FrameAggregation: every frame of the batch in one encoder call
   attentive probe forward / backward                -> AttentiveClassifier (vj_cross_attn_*, wgmma GEMMs, LayerNorm)
   AdamW / GradScaler                                -> FlatAdamW / FlatGradScaler over the probe's flat buffers
   DistributedDataParallel                           -> one averaging all-reduce of the probe's flat gradient per backward
@@ -128,6 +129,11 @@ def main(args_eval, resume_preempt=False):
                          uniform_power=uniform_power, checkpoint_key=checkpoint_key, use_SiLU=use_SiLU,
                          tight_SiLU=tight_SiLU, use_sdpa=use_sdpa)
     if pretrain_frames_per_clip == 1:
+        if not attend_across_segments:
+            # FrameAggregation returns one token sequence per view, which the per-segment loop below cannot take apart
+            # (the reference leaves attend_across_segments=False as a TODO in FrameAggregation.forward)
+            raise ValueError("an image encoder (pretrain frames_per_clip == 1) is evaluated with FrameAggregation, "
+                             "which needs optimization.attend_across_segments: true")
         encoder = FrameAggregation(encoder).to(device)
     else:
         encoder = ClipAggregation(encoder, tubelet_size=tubelet_size,

@@ -98,6 +98,14 @@ int vj_colsum(const void* in, int in_f32, float* out, long long T, int N, long l
 int vj_im2col_tubelets(const float* clips, void* patches, const long long* idx, int B, int C, int T, int H,
                        int W, int tubelet, int patch, int K, void* stream);
 
+/* Positional-embedding resampling for off-size encoder inputs (interpolate_pos_encoding,
+ * src/models/vision_transformer.py:197-246): fp32 in [Nt,Nh,Nw,D] -> fp32 out [T,H,W,D], bit-exact with torch's CPU
+ * F.interpolate(scale_factor=..., align_corners=False).  mode 3: trilinear with per-axis scale factors; mode 2:
+ * bicubic (A = -0.75) over a 2-D grid (Nt = T = 1, scale_t ignored).  Each output extent must be
+ * floor(in * scale); D a multiple of 4, both pointers 16-byte aligned. */
+int vj_pos_interp(const float* in, float* out, int Nt, int Nh, int Nw, int T, int H, int W, int D, double scale_t,
+                  double scale_h, double scale_w, int mode, void* stream);
+
 /* out[b,k,:] = x[b, idx[b,k], :], rows of row_bytes (multiple of 16).  apply_masks, src/masks/utils.py:11-23. */
 int vj_gather_rows(const void* x, void* out, const long long* idx, int B, int N, int K, int row_bytes,
                    void* stream);

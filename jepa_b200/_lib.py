@@ -4,7 +4,7 @@ There is no CPU fallback: if the library is missing or a call fails the caller g
 """
 import ctypes
 import os
-from ctypes import c_char_p, c_float, c_int, c_longlong, c_size_t, c_void_p
+from ctypes import c_char_p, c_double, c_float, c_int, c_longlong, c_size_t, c_void_p
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libvjepa_b200.so")
@@ -31,6 +31,7 @@ SIGNATURES = {
     "vj_layernorm_bwd": (I, [P, P, I, P, P, P, P, P, P, P, P, Z, I, I, P]),
     "vj_colsum": (I, [P, I, P, L, I, L, I, I, I, P]),
     "vj_im2col_tubelets": (I, [P, P, P, I, I, I, I, I, I, I, I, P]),
+    "vj_pos_interp": (I, [P, P, I, I, I, I, I, I, I, c_double, c_double, c_double, I, P]),
     "vj_gather_rows": (I, [P, P, P, I, I, I, I, P]),
     "vj_scatter_rows_add": (I, [P, P, P, I, I, I, I, I, P]),
     "vj_target_ln_gather": (I, [P, P, P, P, P, I, I, I, I, F, F, P]),

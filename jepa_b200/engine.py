@@ -10,6 +10,8 @@ in place (MN-major descriptors, no transposes) and the wgrads reduce straight in
 gradient buffer.
 """
 
+import math
+
 import torch
 
 from . import kernels as K
@@ -259,10 +261,34 @@ class _LayerTaps:
             self.outs.append(y)
 
 
-def encoder_forward(mod, clips, masks, save, final_norm=True, out_layers=None):
+def pos_interp_scales(grid0, grid, video):
+    """scale_factor that interpolate_pos_encoding (vision_transformer.py:197-246) hands to F.interpolate to take the
+    table of token grid `grid0` to `grid`: (T'/Nt, H'/Nh, W'/Nw) for video, sqrt(npatch / N) on both axes for images."""
+    if video:
+        return tuple(g / n for g, n in zip(grid, grid0))
+    s = math.sqrt((grid[1] * grid[2]) / (grid0[1] * grid0[2]))
+    return (1.0, s, s)
+
+
+def encoder_pos(mod, store, grid, dev):
+    """The positional embedding added to the tokens of a `grid` = (T', H', W') input, fp32 [N', D].  At the grid the
+    encoder was built for this is pos_embed itself (no launch); otherwise vj_pos_interp resamples pos_embed into a new
+    buffer on every call, as the reference's interpolate_pos_encoding does (pos_embed may have changed since)."""
+    D = mod.embed_dim
+    n = grid[0] * grid[1] * grid[2]
+    if tuple(grid) == mod.grid:
+        return store.f32("pos_embed").view(n, D)
+    table = store.f32("pos_embed").view(*mod.grid, D)
+    out = _empty((*grid, D), F32, dev)
+    K.pos_interp(table, out, pos_interp_scales(mod.grid, grid, mod.is_video), 3 if mod.is_video else 2)
+    return out.view(n, D)
+
+
+def encoder_forward(mod, clips, masks, save, final_norm=True, out_layers=None, grid=None):
     """VisionTransformer.forward (vision_transformer.py:159-195) for all masks at once.
 
-    clips fp32 [B,3,T,H,W]; masks: None or list of int64 [B,K_i].  Returns (out, saved) where out is
+    clips fp32 [B,3,T,H,W] holding whole patches of the token grid `grid` = (T', H', W') (default: the grid the encoder
+    was built for); masks: None or list of int64 [B,K_i] indexing that grid.  Returns (out, saved) where out is
     bf16 [sum_i B*K_i, D] (normalised if final_norm else the raw residual stream).
     """
     store = mod._store.adopt(mod)
@@ -270,7 +296,8 @@ def encoder_forward(mod, clips, masks, save, final_norm=True, out_layers=None):
     spec = mod._spec
     dev = clips.device
     B = clips.shape[0]
-    N, D = mod.num_patches, mod.embed_dim
+    grid = mod.grid if grid is None else tuple(grid)
+    N, D = grid[0] * grid[1] * grid[2], mod.embed_dim
     P = mod.patch_embed.proj.weight[0].numel()
     weights = gather_block_weights(store, spec, mod._scratch)
     clips = clips.contiguous()
@@ -298,7 +325,7 @@ def encoder_forward(mod, clips, masks, save, final_norm=True, out_layers=None):
         period = 0
     x = _empty((T, D), BF16, dev)
     w_pe = store.bf16("patch_embed.proj.weight").view(D, P)
-    pos = store.f32("pos_embed").view(N, D)
+    pos = encoder_pos(mod, store, grid, dev)
     K.gemm(patches, w_pe, x, bias=store.f32("patch_embed.proj.bias"), epi=K.EPI_ADD, aux=pos, aux_rowmap=rowmap,
            aux_period=period)
     if out_layers is not None:      # frozen-encoder feature taps (evals): list of normalised per-layer outputs

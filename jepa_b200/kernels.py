@@ -130,6 +130,20 @@ def im2col_tubelets(clips, patches, idx, tubelet, patch):
     return patches
 
 
+def pos_interp(table, out, scales, mode):
+    """interpolate_pos_encoding (vision_transformer.py:197-246) on the GPU: table fp32 [Nt, Nh, Nw, D] -> out fp32
+    [T', H', W', D], bit-exact with torch's CPU F.interpolate at scale_factor `scales` = (st, sh, sw).
+    mode 3: trilinear (video); mode 2: bicubic over [1, Nh, Nw, D] (images, st ignored)."""
+    _chk(table, F32, "table"); _chk(out, F32, "out")
+    Nt, Nh, Nw, D = table.shape
+    T, H, W, Do = out.shape
+    if Do != D:
+        raise _lib.VJError(f"pos_interp: width mismatch table={tuple(table.shape)} out={tuple(out.shape)}")
+    st, sh, sw = (float(s) for s in scales)
+    _lib.call("vj_pos_interp", _p(table), _p(out), Nt, Nh, Nw, T, H, W, D, st, sh, sw, int(mode), _s())
+    return out
+
+
 def gather_rows(x, idx, out=None):
     """apply_masks for one mask: x [B,N,D], idx int64 [B,K] -> [B,K,D] (bit-exact row copy)."""
     _chk(x, None, "x"); _chk(idx, torch.int64, "idx")

@@ -125,9 +125,9 @@ def _common_base(tensors):
 # -------------------------------------------------------------------------------------------------
 class _EncoderFn(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, mod, clips, masks, final_norm, *params):
-        save = any(ctx.needs_input_grad[4:])
-        out, sv, _ = engine.encoder_forward(mod, clips, masks, save, final_norm=final_norm)
+    def forward(ctx, mod, clips, masks, final_norm, grid, *params):
+        save = any(ctx.needs_input_grad[5:])
+        out, sv, _ = engine.encoder_forward(mod, clips, masks, save, final_norm=final_norm, grid=grid)
         if save and not final_norm:
             raise RuntimeError("training through the un-normalised encoder output is not supported")
         ctx.mod, ctx.sv = mod, sv
@@ -139,7 +139,7 @@ class _EncoderFn(torch.autograd.Function):
         gflat = engine.encoder_backward(mod, sv, dout)
         ctx.sv = None
         grads = [sv.store.grad_view(gflat, n) if p.requires_grad else None for n, p in mod.named_parameters()]
-        return (None, None, None, None, *grads)
+        return (None, None, None, None, None, *grads)
 
 
 class _PredictorFn(torch.autograd.Function):
@@ -253,39 +253,74 @@ class VisionTransformer(nn.Module):
     def no_weight_decay(self):
         return {}
 
+    @property
+    def grid(self):
+        """Token grid (T', H', W') the positional embedding was built for (T' = 1 for an image encoder)."""
+        g = self.input_size // self.patch_size
+        return (self.num_frames // self.tubelet_size if self.is_video else 1, g, g)
+
+    def token_grid(self, shape):
+        """Token grid of an input of `shape` ([B,C,T,H,W] video, [B,C,H,W] image): (T // tubelet, H // patch,
+        W // patch), flooring like the reference's Conv3d / Conv2d patch embedding.  Raises ValueError for a size the
+        reference's interpolate_pos_encoding (vision_transformer.py:197-246) cannot serve either."""
+        ps = self.patch_size
+        if self.is_video:
+            _, _, T, H, W = shape
+            grid = (T // self.tubelet_size, H // ps, W // ps)
+        else:
+            _, _, H, W = shape
+            grid = (1, H // ps, W // ps)
+        if min(grid) < 1:
+            raise ValueError(f"input {tuple(shape)} is smaller than one {self.tubelet_size}x{ps}x{ps} patch")
+        if grid != self.grid:
+            n0 = self.grid
+            if self.is_video:
+                scales = engine.pos_interp_scales(n0, grid, True)
+                out = tuple(int(n * s) for n, s in zip(n0, scales))
+            else:
+                if grid[1] != grid[2]:
+                    raise ValueError(
+                        f"image of {H}x{W} pixels: a {grid[1]}x{grid[2]} patch grid is not square; the reference's "
+                        "bicubic interpolate_pos_encoding resamples a square table and then fails at x += pos_embed")
+                s = engine.pos_interp_scales(n0, grid, False)[1]
+                out = (1, int(n0[1] * s), int(n0[2] * s))
+            if out != grid:
+                raise ValueError(f"input {tuple(shape)}: interpolate_pos_encoding's scale factors give a {out} table "
+                                 f"for a {grid} token grid (floating-point rounding); the reference fails on it too")
+        return grid
+
     def _check_input(self, x):
+        """Returns (x as a [B,C,T,H,W] clip cropped to whole patches, token grid (T', H', W'))."""
         _require_cuda(x, "VisionTransformer.forward")
         if self.is_video:
             if x.dim() != 5:
                 raise ValueError(f"expected a video batch [B,C,T,H,W], got {tuple(x.shape)}")
-            _, _, T, H, W = x.shape
-            if not (H == self.input_size and W == self.input_size and T == self.num_frames):
-                raise NotImplementedError(
-                    "interpolate_pos_encoding for off-size inputs (vision_transformer.py:197-246) is outside the "
-                    "pre-training path; feed clips at the configured crop_size / num_frames")
-            return x
-        if x.dim() != 4:
+        elif x.dim() != 4:
             raise ValueError(f"expected an image batch [B,C,H,W], got {tuple(x.shape)}")
-        if x.shape[2] != self.input_size or x.shape[3] != self.input_size:
-            raise NotImplementedError("bicubic pos-embed interpolation is outside the pre-training path")
-        return x.unsqueeze(2)
+        grid = self.token_grid(tuple(x.shape))
+        if not self.is_video:
+            x = x.unsqueeze(2)
+        T, H, W = grid[0] * self.tubelet_size, grid[1] * self.patch_size, grid[2] * self.patch_size
+        if x.shape[2:] != (T, H, W):       # the strided patch embedding ignores the remainder
+            x = x[:, :, :T, :H, :W]
+        return x, grid
 
     @torch.no_grad()
     def _forward_out_layers(self, x, masks):
         """vision_transformer.py:183-190 with out_layers set: list of norm(x) after the chosen blocks, each [B, N, D]
         (or [len(masks)*B, K, D]).  Inference only - the evals use it on the frozen encoder."""
-        xv = self._check_input(x)
+        xv, grid = self._check_input(x)
         if masks is not None and len({int(m.shape[1]) for m in masks}) != 1:
             raise ValueError("out_layers with masks of different sizes cannot be concatenated along batch")
-        outs, _, _ = engine.encoder_forward(self, xv, masks, save=False, out_layers=self.out_layers)
+        outs, _, _ = engine.encoder_forward(self, xv, masks, save=False, out_layers=self.out_layers, grid=grid)
         B = xv.shape[0] * (1 if masks is None else len(masks))
         return [o.view(B, -1, self.embed_dim) for o in outs]
 
     def forward_multi(self, x, masks, final_norm=True):
         """All masks in one fused pass.  Returns list of [B, K_i, D] bf16 views (one per mask)."""
-        x = self._check_input(x)
+        x, grid = self._check_input(x)
         params = [p for _, p in self.named_parameters()]
-        out = _EncoderFn.apply(self, x, list(masks), final_norm, *params)
+        out = _EncoderFn.apply(self, x, list(masks), final_norm, grid, *params)
         return _token_views(out, x.shape[0], [int(m.shape[1]) for m in masks])
 
     def forward(self, x, masks=None):
@@ -299,10 +334,10 @@ class VisionTransformer(nn.Module):
         if self.out_layers is not None:
             return self._forward_out_layers(x, masks)
         if masks is None:
-            xv = self._check_input(x)
+            xv, grid = self._check_input(x)
             params = [p for _, p in self.named_parameters()]
-            out = _EncoderFn.apply(self, xv, None, True, *params)
-            return out.view(xv.shape[0], self.num_patches, self.embed_dim)
+            out = _EncoderFn.apply(self, xv, None, True, grid, *params)
+            return out.view(xv.shape[0], grid[0] * grid[1] * grid[2], self.embed_dim)
         sizes = {int(m.shape[1]) for m in masks}
         if len(sizes) != 1:
             raise ValueError("VisionTransformer.forward(x, masks=[...]) concatenates along batch and needs equal K; "

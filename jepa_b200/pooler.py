@@ -1,6 +1,6 @@
 """Frozen-encoder evaluation side of V-JEPA on the sm_90a kernels (SURVEY section 8, row f4): the attentive probe
 (src/models/attentive_pooler.py:21-136, CrossAttention / CrossAttentionBlock of src/models/utils/modules.py:122-182) and
-the clip aggregation wrapper (evals/video_classification_frozen/utils.py:86-159).
+the clip and frame aggregation wrappers (evals/video_classification_frozen/utils.py:23-159).
 
 Same constructor arguments, parameter names, initialisation and `state_dict` keys as the reference, so a probe checkpoint
 written by the reference's eval loop loads here unchanged.  Everything runs on the hand-written kernels (LayerNorm, wgmma
@@ -22,7 +22,7 @@ import torch
 import torch.nn as nn
 
 from . import kernels as K
-from .models import MLP
+from .models import MLP, VisionTransformer
 from .params import FlatParamStore
 from .pos_embs import get_1d_sincos_pos_embed
 from .tensors import apply_masks, trunc_normal_
@@ -397,6 +397,49 @@ class AttentiveClassifier(nn.Module):
     def forward(self, x):
         """x [B, S, D] encoder tokens -> logits fp32 [B, num_classes]."""
         return _run_probe(self, self.pooler, x, head=True)
+
+
+class FrameAggregation(nn.Module):
+    """An image encoder evaluated on video (evals/video_classification_frozen/utils.py:23-83, used when the pre-training
+    config has frames_per_clip == 1): every frame of every segment and view goes through the encoder in ONE batch, and
+    each view comes back as one sequence [B, frames * segments * N, D], segments strung together along time - optionally
+    tagged with the 1-D sin-cos position of each frame's clip index.  As in the reference, attend_across_segments is
+    accepted but has no effect: the output is always one sequence per view.
+
+    `model` must be an image encoder of jepa_b200.models (VisionTransformer with num_frames == 1), the encoder that runs
+    the frames on the kernels; any other module (a video encoder, an eager PyTorch model) raises NotImplementedError."""
+
+    def __init__(self, model, max_frames=10000, use_pos_embed=False, attend_across_segments=False):
+        super().__init__()
+        if not isinstance(model, VisionTransformer) or model.is_video:
+            what = "a video encoder (num_frames > 1)" if isinstance(model, VisionTransformer) else type(model).__name__
+            raise NotImplementedError(
+                f"FrameAggregation runs an image encoder of jepa_b200.models (VisionTransformer, num_frames=1) frame by "
+                f"frame on the sm_90a kernels; wrapping {what} is not implemented")
+        self.model = model
+        self.embed_dim = model.embed_dim
+        self.num_heads = model.num_heads
+        self.attend_across_segments = attend_across_segments
+        self.pos_embed = None
+        if use_pos_embed:
+            table = torch.from_numpy(get_1d_sincos_pos_embed(self.embed_dim, max_frames)).float()
+            self.pos_embed = nn.Parameter(table.unsqueeze(0), requires_grad=False)
+
+    def forward(self, x, clip_indices=None):
+        """x: list (segments) of lists (views) of [B, C, T, H, W]; returns per view [B, segments * T * N, D]."""
+        n_views = len(x[0])
+        clips = torch.cat([torch.cat(views, dim=0) for views in x], dim=2)     # views on batch, segments along time
+        VB, C, T, H, W = clips.shape
+        tokens = self.model(clips.transpose(1, 2).reshape(VB * T, C, H, W))  # frame-major within each clip
+        N, D = tokens.shape[1], tokens.shape[2]
+        tokens = tokens.view(VB, T * N, D)
+        B = VB // n_views
+        tags = None
+        if self.pos_embed is not None and clip_indices is not None:
+            rows = apply_masks(self.pos_embed.expand(B, -1, -1), list(clip_indices), concat=False)    # [B, T_s, D] each
+            tags = torch.cat(rows, dim=1).unsqueeze(2).expand(-1, -1, N, -1).flatten(1, 2)
+        views = [tokens[v * B:(v + 1) * B] for v in range(n_views)]
+        return views if tags is None else [o + tags.to(o.dtype) for o in views]
 
 
 class ClipAggregation(nn.Module):

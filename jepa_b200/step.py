@@ -33,9 +33,9 @@ def forward_target(target_encoder, clips, masks_pred):
     Returns a list of fp32 [B, Kp_i, D] views of one contiguous buffer.
     """
     bb = unwrap(target_encoder)
-    x = bb._check_input(clips)
-    raw, _, _ = engine.encoder_forward(bb, x, None, save=False, final_norm=False)
-    B, N, D = x.shape[0], bb.num_patches, bb.embed_dim
+    x, grid = bb._check_input(clips)
+    raw, _, _ = engine.encoder_forward(bb, x, None, save=False, final_norm=False, grid=grid)
+    B, N, D = x.shape[0], grid[0] * grid[1] * grid[2], bb.embed_dim
     raw = raw.view(B, N, D)
     store = bb._store
     sizes = [int(m.shape[1]) for m in masks_pred]
