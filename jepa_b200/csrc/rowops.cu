@@ -411,6 +411,21 @@ __global__ void __launch_bounds__(256) lp_loss_bwd_kernel(const __nv_bfloat16* _
   }
 }
 
+// Mean and unbiased variance of one (b, d) column of z over its K tokens (stride D), in two passes: the one-pass
+// (sum v^2 - K mean^2) form cancels when |mean| >> std, which are exactly the channels where relu(1 - pstd) is active.
+// The squared deviations are summed in double: an fp32 running sum over a few thousand tokens drifts by ~1e-5.
+VJ_DEVINL void token_mean_var(const __nv_bfloat16* __restrict__ p, int K, int D, float& mean, float& var) {
+  float s = 0.f;
+  for (int k = 0; k < K; ++k) s += __bfloat162float(p[(long long)k * D]);
+  mean = s / K;
+  double ss = 0.0;
+  for (int k = 0; k < K; ++k) {
+    const double dv = __bfloat162float(p[(long long)k * D]) - mean;
+    ss += dv * dv;
+  }
+  var = float(ss / (K - 1));
+}
+
 // Backward of the variance regulariser (train.py:448-449,458-459) for one mask:
 //   loss_reg = mean_{b,d} relu(1 - pstd[b,d]),  pstd = sum_i w * sqrt(var_unbiased_k(z_i[b,k,d]) + eps)
 //   d loss_reg / d z_i[b,k,d] = -[pstd < 1] / (B D) * w * (z - mean_k z) / ((K - 1) * sqrt(var + eps))
@@ -424,14 +439,8 @@ __global__ void __launch_bounds__(128) token_std_bwd_kernel(const __nv_bfloat16*
   if (d >= D) return;
   const __nv_bfloat16* p = z + (long long)b * K * D + d;
   __nv_bfloat16* q = dz + (long long)b * K * D + d;
-  float s = 0.f, ss = 0.f;
-  for (int k = 0; k < K; ++k) {
-    const float v = __bfloat162float(p[(long long)k * D]);
-    s += v;
-    ss += v * v;
-  }
-  const float mean = s / K;
-  const float var = fmaxf((ss - K * mean * mean) / (K - 1), 0.f);
+  float mean, var;
+  token_mean_var(p, K, D, mean, var);
   const float g = scale * (gscale ? *gscale : 1.0f);
   const float c = pstd_total[(long long)b * D + d] < 1.0f ? -g * weight / ((float)B * D * (K - 1) * sqrtf(var + eps)) : 0.f;
   for (int k = 0; k < K; ++k) q[(long long)k * D] = __float2bfloat16(c * (__bfloat162float(p[(long long)k * D]) - mean));
@@ -443,16 +452,8 @@ __global__ void __launch_bounds__(256) token_std_kernel(const __nv_bfloat16* __r
   const int d = blockIdx.x * blockDim.x + threadIdx.x;
   const int b = blockIdx.y;
   if (d >= D) return;
-  float s = 0.f, ss = 0.f;
-  const __nv_bfloat16* p = z + (long long)b * K * D + d;
-  for (int k = 0; k < K; ++k) {
-    const float v = __bfloat162float(p[(long long)k * D]);
-    s += v;
-    ss += v * v;
-  }
-  const float mean = s / K;
-  float var = (ss - K * mean * mean) / (K - 1);
-  var = fmaxf(var, 0.f);
+  float mean, var;
+  token_mean_var(z + (long long)b * K * D + d, K, D, mean, var);
   pstd[(long long)b * D + d] += weight * sqrtf(var + eps);
 }
 

@@ -22,6 +22,9 @@ VITL_2B = dict(model_name='vit_large', crop_size=224, patch_size=16, num_frames=
                pred_depth=2, pred_embed_dim=384, depth=2, heads=16, embed_dim=1024, mask_batch=32)
 VITH_2B = dict(model_name='vit_huge', crop_size=224, patch_size=16, num_frames=16, tubelet_size=2, batch=1,
                pred_depth=2, pred_embed_dim=384, depth=2, heads=16, embed_dim=1280, mask_batch=24)
+# ViT-g/16: 16 heads of 88 (padded to 128), MLP 6144 = 1408 * 48/11, the only shipped encoder wider than 1280; C2's masks
+VITG_2B = dict(model_name='vit_giant', crop_size=224, patch_size=16, num_frames=16, tubelet_size=2, batch=1,
+               pred_depth=2, pred_embed_dim=384, depth=2, heads=16, embed_dim=1408, mlp_ratio=48 / 11, mask_batch=32)
 
 
 def cfg_masks(cfg, batch):
@@ -45,7 +48,7 @@ def _shapes(depth, pred_depth, cfg=C1):
     import torch.nn as nn
     enc = VisionTransformer(img_size=cfg["crop_size"], patch_size=cfg["patch_size"], num_frames=cfg["num_frames"],
                             tubelet_size=cfg["tubelet_size"], embed_dim=cfg["embed_dim"], depth=depth, num_heads=cfg["heads"],
-                            mlp_ratio=4, qkv_bias=True, norm_layer=partial(nn.LayerNorm, eps=1e-6), uniform_power=True)
+                            mlp_ratio=cfg.get("mlp_ratio", 4), qkv_bias=True, norm_layer=partial(nn.LayerNorm, eps=1e-6), uniform_power=True)
     pred = vit_predictor(img_size=cfg["crop_size"], use_mask_tokens=True, patch_size=cfg["patch_size"],
                          num_frames=cfg["num_frames"], tubelet_size=cfg["tubelet_size"], embed_dim=cfg["embed_dim"],
                          predictor_embed_dim=cfg["pred_embed_dim"], depth=pred_depth, num_heads=cfg["heads"],

@@ -15,7 +15,7 @@ import pytest
 import torch
 
 from common import synth_clips
-from parity_util import (TOL_ACT, VITH_2B, VITL_2B, c1_masks, compare_step, rel_l2, run_c1_step_cuda, run_c1_step_oracle)
+from parity_util import (TOL_ACT, VITG_2B, VITH_2B, VITL_2B, c1_masks, compare_step, rel_l2, run_c1_step_cuda, run_c1_step_oracle)
 
 pytestmark = pytest.mark.gpu
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -100,7 +100,7 @@ def test_linear_backward_gemms(dev):
 
 
 # --------------------------------------------------------------------------------------------- rows
-@pytest.mark.parametrize("D", [192, 384, 1024, 1280])
+@pytest.mark.parametrize("D", [192, 384, 768, 1024, 1280, 1408, 2048])
 def test_layernorm_fwd_bwd(dev, D):
     from jepa_b200 import kernels as Kn
     from oracle import vjepa_oracle as O
@@ -416,10 +416,10 @@ def test_c1_step_full_vs_oracle_and_golden(dev, golden_dir):
         assert torch.equal(got["ema"][n].reshape(-1)[:32], ref_slice), n
 
 
-@pytest.mark.parametrize("cfg", [VITL_2B, VITH_2B], ids=["vitl16_2blocks", "vith16_2blocks"])
+@pytest.mark.parametrize("cfg", [VITL_2B, VITH_2B, VITG_2B], ids=["vitl16_2blocks", "vith16_2blocks", "vitg16_2blocks"])
 def test_baseline_width_step_vs_oracle(dev, cfg):
     """SURVEY 8c(ii): a 2+2-block slice of the BASELINE networks at FULL width / heads / sequence lengths (ViT-L: D=1024,
-    16 heads of 64; ViT-H: D=1280, 16 heads of 80 -> 128; predictor 384 / 16 heads of 24 -> 32; N=1568 target tokens,
+    16 heads of 64; ViT-H: D=1280, 16 heads of 80 -> 128; ViT-g: D=1408, 16 heads of 88 -> 128, MLP 6144; predictor 384 / 16 heads of 24 -> 32; N=1568 target tokens,
     C2's seeded masks Ke=[360,48] Kp=[824,1144]), one clip, against the fp32 CPU oracle: target / context / predictor
     outputs, loss, every parameter gradient (BN=256 GEMM tiles, split-K wgrads at these K), EMA bit-exact."""
     got = run_c1_step_cuda(dev, cfg=cfg)
