@@ -3,6 +3,8 @@
 PyTorch is only the allocator / stream provider here; every op below is one of our own sm_90a
 kernels.  All functions enqueue on torch's current stream and never synchronise.
 """
+import ctypes
+
 import torch
 
 from . import _lib
@@ -274,6 +276,18 @@ def ema_update(k_flat, q_flat, m):
 def adamw_step(p, g, m, v, lr, beta1, beta2, eps, wd, step, inv_scale=None, found_inf=None):
     _lib.call("vj_adamw_step", _p(p), _p(g), _p(m), _p(v), p.numel(), float(lr), float(beta1), float(beta2),
               float(eps), float(wd), int(step), _p(inv_scale), _p(found_inf), _s())
+
+
+def adamw_flat(p, g, m, v, group_ids, lr, wd, beta1, beta2, eps, step_dev, shadow, inv_scale=None, found_inf=None):
+    """AdamW over a whole flat buffer in one launch: group_ids (uint8 per 64 elements) pick (lr[i], wd[i]) of at most 4
+    groups, id 255 is skipped; step_dev is the device step counter, shadow receives the bf16 copy of the update."""
+    _chk(p, F32, "p"); _chk(g, F32, "g"); _chk(m, F32, "m"); _chk(v, F32, "v")
+    _chk(group_ids, torch.uint8, "group_ids"); _chk(step_dev, F32, "step_dev"); _chk(shadow, BF16, "shadow")
+    lr4 = (ctypes.c_float * 4)(*map(float, lr))      # unused entries stay 0
+    wd4 = (ctypes.c_float * 4)(*map(float, wd))
+    _lib.call("vj_adamw_flat", _p(p), _p(g), _p(m), _p(v), _p(group_ids), p.numel(), ctypes.cast(lr4, ctypes.c_void_p),
+              ctypes.cast(wd4, ctypes.c_void_p), float(beta1), float(beta2), float(eps), 0, _p(inv_scale), _p(found_inf),
+              _p(step_dev), _p(shadow), _s())
 
 
 def sumsq(x, out):

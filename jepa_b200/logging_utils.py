@@ -80,39 +80,20 @@ def _to_floats(tensors):
     return torch.stack([t.float().reshape(()) for t in tensors]).tolist()
 
 
-def _flat_grad_sumsq(named):
-    """Per-tensor sum of squares of the gradients of `named` [(name, param)] through the segmented kernel, when all of
-    them are slices of ONE flat gradient buffer of their FlatParamStore.  Uses the statistics the unscale pass of this
-    step already produced when they are still current, else one stats-only pass.  Returns {name: device scalar} or None."""
-    from . import kernels as K
-    store = None
-    for _, p in named:
-        st = getattr(p, "_vj_store", None)
-        if st is None or (store is not None and st is not store) or not st.owns(p):
-            return None
-        store = st
-    if store is None:
+def _flat_grad_sumsq(params):
+    """(store, gradient buffer, per-tensor sums of squares, rows) when every parameter of `params` (all with a .grad) is
+    a trainable member of ONE FlatParamStore and the gradients are slices of its flat buffer, else None.  params[i]'s
+    sum of squares is sumsq[rows[i]]; the sums are those the unscale pass of this step left when still current."""
+    store = getattr(params[0], "_vj_store", None)
+    if store is None or not all(getattr(p, "_vj_store", None) is store and store.owns(p) for p in params):
         return None
-    base = None
-    for _, p in named:
-        g = p.grad
-        if g is None or g.dtype != torch.float32 or not g.is_contiguous():
-            return None
-        b = g.data_ptr() - 4 * store.offsets[p._vj_name][0]
-        if base is None:
-            base = b
-        elif b != base:
-            return None
-    seg, names = store.segments()
-    cache = getattr(store, "_grad_sumsq", None)
-    if cache is not None and cache[0] == base and cache[1] == getattr(store, "_grad_gen", 0):
-        sumsq = cache[2]
-    else:
-        sumsq = torch.zeros(len(names), dtype=torch.float32, device=store.flat.device)
-        from . import _lib
-        _lib.call("vj_grad_unscale_stats", base, seg.data_ptr(), store.total, None, None, sumsq.data_ptr(), 0, K._s())
-    index = {n: i for i, n in enumerate(names)}
-    return {p._vj_name: (sumsq, index[p._vj_name]) for _, p in named if p._vj_name in index}
+    gflat = store.grad_buffer(params)
+    if gflat is None:
+        return None
+    index = {n: i for i, n in enumerate(store.segments()[1])}
+    if not all(p._vj_name in index for p in params):
+        return None
+    return store, gflat, store.grad_sumsq(gflat), [index[p._vj_name] for p in params]
 
 
 def grad_logger(named_params):
@@ -123,11 +104,11 @@ def grad_logger(named_params):
     names = [n for n, _ in named]
     norms = []
     if named:
-        flat = _flat_grad_sumsq(named) if named[0][1].is_cuda else None
-        if flat is not None and len(flat) == len(named):
-            sumsq = next(iter(flat.values()))[0]
+        flat = _flat_grad_sumsq([p for _, p in named]) if named[0][1].is_cuda else None
+        if flat is not None:
+            _, _, sumsq, rows = flat
             host = sumsq.sqrt().tolist()                      # the only host sync
-            norms = [host[flat[p._vj_name][1]] for _, p in named]
+            norms = [host[i] for i in rows]
         else:
             norms = _to_floats(list(torch._foreach_norm([p.grad.data for _, p in named])))
     stats = AverageMeter()
@@ -148,23 +129,19 @@ def adamw_logger(optimizer):
     """Mean |exp_avg| and |exp_avg_sq| per state tensor -> AverageMeters (logging.py:108-118).  FlatAdamW keeps both
     moments of a backbone in one flat buffer each: two segmented |x| reductions per backbone, one device->host copy."""
     from . import kernels as K
+    from .optim import FlatAdamW
     vals1, vals2 = [], []
-    flat_states = getattr(optimizer, "_flat", None)
     covered = set()
-    if flat_states:
+    if isinstance(optimizer, FlatAdamW):
         parts = []
-        for st in flat_states.values():
-            store = st["store"]
+        for store, m, v, params in optimizer.flat_moments():
             seg, names = store.segments()
             out = torch.zeros(2, len(names), dtype=torch.float32, device=store.flat.device)
-            K.seg_abs_sum(st["m"], seg, out[0])
-            K.seg_abs_sum(st["v"], seg, out[1])
+            K.seg_abs_sum(m, seg, out[0])
+            K.seg_abs_sum(v, seg, out[1])
             numel = torch.tensor([store.offsets[n][1] for n in names], dtype=torch.float32)
             parts.append((out, numel))
-            for n, p in store._params:
-                if p in optimizer.state and optimizer.state[p].get("exp_avg") is not None and \
-                        optimizer.state[p]["exp_avg"].data_ptr() == st["m"].data_ptr() + 4 * store.offsets[n][0]:
-                    covered.add(p)
+            covered |= params
         for out, numel in parts:
             host = out.cpu()                                  # one copy per backbone
             vals1 += (host[0] / numel).tolist()

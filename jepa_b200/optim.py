@@ -13,11 +13,8 @@ Anything else falls back to one `vj_adamw_step` launch per tensor.  A trainable 
 (the attentive probe's `proj`, which the reference never applies) is treated as torch.optim.AdamW treats it: it is not
 updated and gets no optimizer state.
 """
-import ctypes
-
 import torch
 
-from . import _lib
 from . import kernels as K
 
 
@@ -65,15 +62,24 @@ class FlatAdamW(torch.optim.Optimizer):
         """Members the flat step updates: trainable and with a gradient this step (torch.optim.AdamW skips the rest)."""
         return p.requires_grad and p.grad is not None
 
+    def _in_flat_moments(self, st, name, p):
+        """True if p's exp_avg is still its slice of the flat moment buffer of `st` (load_state_dict replaces it)."""
+        ea = self.state.get(p, {}).get("exp_avg")
+        return ea is not None and ea.data_ptr() == st["m"].data_ptr() + 4 * st["store"].offsets[name][0]
+
+    def flat_moments(self):
+        """[(store, m, v, params)]: the flat first / second moment buffers of each store stepped by one launch, and the
+        parameters whose exp_avg / exp_avg_sq are still slices of them."""
+        return [(st["store"], st["m"], st["v"], {p for n, p in st["store"]._params if self._in_flat_moments(st, n, p)})
+                for st in self._flat.values()]
+
     def _flat_state(self, store, members):
         key = (store.flat.data_ptr(), store.total, tuple((gi, id(p), self._stepped(p)) for gi, p in members))
         st = self._flat.get(id(store))
         if st is not None and st["key"] == key:
             p0 = next(p for _, p in members if self._stepped(p))   # frozen / gradient-less members carry no state
-            off0 = store.offsets[p0._vj_name][0]
-            ea = self.state.get(p0, {}).get("exp_avg")
-            if ea is not None and ea.data_ptr() == st["m"].data_ptr() + 4 * off0:
-                return st          # state still aliases the flat moment buffers (not replaced by load_state_dict)
+            if self._in_flat_moments(st, p0._vj_name, p0):
+                return st
         dev = store.flat.device
         gid = torch.full((store.total // 64,), 255, dtype=torch.uint8)
         for gi, p in members:
@@ -102,25 +108,6 @@ class FlatAdamW(torch.optim.Optimizer):
         self._flat[id(store)] = st
         return st
 
-    @staticmethod
-    def _flat_grad_base(store, members):
-        """Device pointer of the flat gradient buffer if every member's .grad is its slice of one buffer.  Members without
-        a gradient are skipped (not stepped, see _stepped)."""
-        base = None
-        for _, p in members:
-            g = p.grad
-            if g is None:
-                continue
-            if g.dtype != torch.float32 or not g.is_contiguous():
-                return None
-            off = store.offsets[p._vj_name][0]
-            b = g.data_ptr() - 4 * off
-            if base is None:
-                base = b
-            elif b != base:
-                return None
-        return base
-
     # ------------------------------------------------------------------------------------------ GradScaler hook
     @torch.no_grad()
     def unscale_flat_(self, inv_scale, found_inf):
@@ -128,28 +115,13 @@ class FlatAdamW(torch.optim.Optimizer):
         non-finite flag and leaves per-tensor sums of squares behind for grad_logger / clip_grad_norm_ (no host sync).
         Returns the parameters it did not cover (torch's foreach path handles those)."""
         by_store, leftovers = self._flat_plan()
-        self._grad_stats = {}
         for store, members in by_store.values():
-            base = self._flat_grad_base(store, members)
-            if base is None:
+            gflat = store.grad_buffer(p for _, p in members)
+            if gflat is None:
                 leftovers.extend(members)
-                continue
-            seg, names = store.segments()
-            sumsq = torch.zeros(len(names), dtype=torch.float32, device=store.flat.device)
-            _lib.call("vj_grad_unscale_stats", base, seg.data_ptr(), store.total, K._p(inv_scale), K._p(found_inf),
-                      sumsq.data_ptr(), 1, K._s())
-            self._grad_stats[id(store)] = (store, base, sumsq, names)
-            store._grad_sumsq = (base, getattr(store, "_grad_gen", 0), sumsq)   # reused by grad_logger / clip_grad_norm_
+            else:
+                store.grad_sumsq(gflat, inv_scale, found_inf)
         return [p for _, p in leftovers if p.grad is not None]
-
-    def grad_stats_for(self, store):
-        """(sumsq tensor, names) left by the last unscale_flat_ for this store, or None."""
-        hit = getattr(self, "_grad_stats", {}).get(id(store))
-        return None if hit is None else (hit[2], hit[3])
-
-    def zero_grad(self, set_to_none=True):
-        self._grad_stats = {}
-        return super().zero_grad(set_to_none=set_to_none)
 
     @torch.no_grad()
     def step(self, closure=None):
@@ -167,19 +139,17 @@ class FlatAdamW(torch.optim.Optimizer):
 
         by_store, leftovers = self._flat_plan()
         for store, members in by_store.values():
-            base = self._flat_grad_base(store, members)
+            gflat = store.grad_buffer(p for _, p in members)
             # parameters of the store that are NOT optimised here (frozen ones) stay untouched: group id 255
-            if base is None:
+            if gflat is None:
                 leftovers.extend(members)
                 continue
             st = self._flat_state(store, members)
-            lr4 = (ctypes.c_float * 4)(*[float(g['lr']) for g in self.param_groups[:4]] + [0.0] * (4 - min(4, len(self.param_groups))))
-            wd4 = (ctypes.c_float * 4)(*[float(g['weight_decay']) for g in self.param_groups[:4]] + [0.0] * (4 - min(4, len(self.param_groups))))
+            groups = self.param_groups[:4]
             beta1, beta2 = self.param_groups[0]['betas']
-            _lib.call("vj_adamw_flat", store.flat.data_ptr(), base, st["m"].data_ptr(), st["v"].data_ptr(),
-                      st["gid"].data_ptr(), store.total, ctypes.cast(lr4, ctypes.c_void_p), ctypes.cast(wd4, ctypes.c_void_p),
-                      float(beta1), float(beta2), float(self.param_groups[0]['eps']), 0,
-                      K._p(inv_scale), K._p(found_inf), st["step"].data_ptr(), store.shadow.data_ptr(), K._s())
+            K.adamw_flat(store.flat, gflat, st["m"], st["v"], st["gid"], [g['lr'] for g in groups],
+                         [g['weight_decay'] for g in groups], beta1, beta2, self.param_groups[0]['eps'], st["step"],
+                         store.shadow, inv_scale, found_inf)
             store.mark_shadow_fresh()     # the kernel wrote next step's bf16 operands with the update (if not skipped,
                                           # and if skipped the previous shadow is still the right one)
 

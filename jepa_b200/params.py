@@ -38,6 +38,7 @@ class FlatParamStore:
         self._shadow_fresh = False   # set by the kernels that emit the bf16 shadow together with a parameter update
         self._shadow_complete = False   # a full cast has filled every element of the shadow at least once
         self._seg = None             # uint16 per 64-element block -> index into named parameters (0xFFFF: frozen / padding)
+        self._grad_sumsq = None      # (gradient buffer address, per-tensor sums of squares the unscale pass left behind)
 
     def __deepcopy__(self, memo):
         return FlatParamStore()  # copies re-adopt their own (deep-copied) parameters lazily
@@ -134,10 +135,52 @@ class FlatParamStore:
         o, n, shape = self.offsets[name]
         return self.flat[o:o + n].view(shape)
 
+    # -- the flat gradient buffer ----------------------------------------------------------------
     def new_grad_buffer(self):
-        self._grad_gen = getattr(self, "_grad_gen", 0) + 1     # invalidates cached per-tensor gradient statistics
+        self.grads_changed()
         return torch.zeros(self.total, dtype=torch.float32, device=self.flat.device)
 
     def grad_view(self, gflat, name):
         o, n, shape = self.offsets[name]
         return gflat[o:o + n].view(shape)
+
+    def grad_buffer(self, params):
+        """The flat fp32 [total] gradient buffer whose slices the .grads of `params` (members of this store) are, or None.
+        Every parameter that has a .grad must be fp32, contiguous and sit at its offset in one buffer; parameters without
+        a .grad are skipped, and None is returned when none has one."""
+        base = first = None
+        for p in params:
+            g = p.grad
+            if g is None:
+                continue
+            if g.dtype != torch.float32 or not g.is_contiguous():
+                return None
+            off = self.offsets[p._vj_name][0]
+            if first is None:
+                base, first = g.data_ptr() - 4 * off, (g, off)
+            elif g.data_ptr() - 4 * off != base:
+                return None
+        if first is None:
+            return None
+        g, off = first
+        start = g.storage_offset() - off
+        if start < 0 or 4 * (start + self.total) > g.untyped_storage().nbytes():
+            return None
+        return torch.as_strided(g, (self.total,), (1,), storage_offset=start)
+
+    def grad_sumsq(self, gflat, inv_scale=None, found_inf=None):
+        """Per-tensor sums of squares of the gradient buffer `gflat`, one per trainable tensor (in segments()[1] order).
+        With inv_scale (GradScaler's unscale) the same pass unscales gflat in place and raises found_inf on a non-finite
+        value; later calls reuse those sums until grads_changed().  Without, one stats-only pass when nothing is cached."""
+        if inv_scale is None and self._grad_sumsq is not None and self._grad_sumsq[0] == gflat.data_ptr():
+            return self._grad_sumsq[1]
+        seg, names = self.segments()
+        sumsq = torch.zeros(len(names), dtype=torch.float32, device=gflat.device)
+        K.grad_unscale_stats(gflat, seg, sumsq, inv_scale, found_inf, write_back=inv_scale is not None)
+        if inv_scale is not None:
+            self._grad_sumsq = (gflat.data_ptr(), sumsq)     # the address only: the cache keeps no buffer alive
+        return sumsq
+
+    def grads_changed(self):
+        """The gradient buffer was replaced or written: statistics cached for it are stale."""
+        self._grad_sumsq = None

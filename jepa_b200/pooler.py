@@ -47,21 +47,11 @@ def _store_of(module, anchor):
 def _grad_buffer(store, members):
     """The flat gradient buffer of this step: the one the members' .grad already alias (an earlier probe call of the
     same step), else a new zero buffer."""
-    base = None
-    for n, p in members:
-        g = p.grad
-        if g is None or g.dtype != F32 or not g.is_contiguous():
-            base = None
-            break
-        b = g.data_ptr() - 4 * store.offsets[n][0]
-        if base is not None and b != base:
-            base = None
-            break
-        base = b
-    if base is not None:
-        store._grad_gen = getattr(store, "_grad_gen", 0) + 1     # the buffer changes: cached statistics are stale
-        g0 = members[0][1].grad
-        return torch.as_strided(g0, (store.total,), (1,), storage_offset=g0.storage_offset() - store.offsets[members[0][0]][0])
+    if all(p.grad is not None for _, p in members):
+        gflat = store.grad_buffer(p for _, p in members)
+        if gflat is not None:
+            store.grads_changed()
+            return gflat
     gflat = store.new_grad_buffer()
     for n, p in members:
         p.grad = store.grad_view(gflat, n)

@@ -164,19 +164,15 @@ def clip_grad_norm_(module, max_norm):
     clipping is needed.  Returns the total norm as a device scalar (float() it like the reference does)."""
     from .logging_utils import _flat_grad_sumsq
     bb = unwrap(module)
-    named = [(n, p) for n, p in bb.named_parameters() if p.grad is not None]
-    if not named:
+    params = [p for p in bb.parameters() if p.grad is not None]
+    if not params:
         return torch.zeros((), device=next(bb.parameters()).device)
-    flat = _flat_grad_sumsq(named)
-    if flat is None or len(flat) != len(named):
-        return torch.nn.utils.clip_grad_norm_([p for _, p in named], max_norm)
-    sumsq = next(iter(flat.values()))[0]
-    store = named[0][1]._vj_store
+    flat = _flat_grad_sumsq(params)
+    if flat is None:
+        return torch.nn.utils.clip_grad_norm_(params, max_norm)
+    store, gflat, sumsq, _ = flat
     out = torch.empty(2, dtype=torch.float32, device=sumsq.device)
     K.clip_coef(sumsq, max_norm, out[0:1], out[1:2])
-    p0 = named[0][1]
-    base_off = store.offsets[p0._vj_name][0]
-    gflat = torch.as_strided(p0.grad, (store.total,), (1,), storage_offset=p0.grad.storage_offset() - base_off)
     K.scale_flat(gflat, out[1:2])
-    store._grad_sumsq = None          # the cached statistics describe the unclipped gradients
+    store.grads_changed()
     return out[0]
