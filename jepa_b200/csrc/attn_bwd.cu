@@ -5,15 +5,17 @@
 //   dQ = scale dS K, dK = scale dS^T Q.
 // Three kernels:
 //   attn_delta_kernel  : delta[h,t] = sum_d dO[t,h,d] O[t,h,d]                      (HBM-bound)
-//   attn_bwd_dkv_kernel: one CTA per 128-key tile (two consumer warpgroups of 64 keys), loops over 64-query tiles;
+//   attn_bwd_dkv_kernel: one CTA per tile of 64 * NWG keys (NWG consumer warpgroups of 64 keys), loops over 64-query tiles;
 //                        computes S^T = K Q^T and dP^T = V dO^T directly in the transposed orientation so P^T / dS^T are
 //                        register A operands of dV += P^T dO and dK += dS^T Q, both accumulated in registers across the loop.
-//   attn_bwd_dq_kernel : one CTA per 128-query tile, loops over 64-key tiles; dQ += dS K in registers.
+//   attn_bwd_dq_kernel : one CTA per tile of 64 * NWG queries, loops over 64-key tiles; dQ += dS K in registers.
 // Both loop kernels are warp-specialised like the forward: warpgroup 0 is the producer (one warp: TMA of the streamed
 // tiles into a 3-stage ring with full / empty mbarriers; for dK/dV it also stages the streamed queries' lse2 / delta in
-// shared memory, so the exps never wait on global loads), warpgroups 1-2 are the consumers, 64 resident rows each.
-// Without a CTA-wide barrier per tile the two consumers drift apart, so one's P / dS elementwise work runs under the
-// other's MMAs.  (Explicit ping-pong through named barriers, and issuing the next S / dP ahead of the current gradient
+// shared memory, so the exps never wait on global loads), warpgroups 1..NWG are the consumers, 64 resident rows each; a
+// consumer whose rows all lie past the sequence's end exits at once.  Without a CTA-wide barrier per tile the consumers
+// drift apart, so one's P / dS elementwise work runs under the others' MMAs.  NWG is chosen per (kernel, head dim)
+// (bwd_nwg): more warpgroups put more independent chains on each warp scheduler and share each streamed tile among more
+// resident rows.  (Explicit ping-pong through named barriers, and issuing the next S / dP ahead of the current gradient
 // MMAs, were both measured slower on these short-K tiles.)  The arithmetic per resident row is unchanged by the schedule.
 // P is recomputed from the forward's log2-domain LSE.  Same qkv / O layouts as attn_fwd.cu; the
 // gradient dqkv has the qkv layout [T, 3*H*HD] so the qkv wgrad/dgrad GEMMs consume it directly.
@@ -24,7 +26,6 @@
 
 namespace vj {
 
-constexpr int kBwdThreads = 384;
 constexpr int kBwdStream = 64;   // rows of the streamed (query or key) tiles
 constexpr int kBwdStages = 3;
 
@@ -37,12 +38,17 @@ struct AttnBwdParams {
   float scale, scale_log2;
 };
 
-template <int HD>
+// Consumer warpgroups per CTA, measured per (kernel, head dim) (DESIGN section 6).  Two at hd 128, and for dK / dV at
+// hd 64, where the two accumulators do not fit three warpgroups' register budget without spills (nor at hd 32 in four).
+template <int HD, bool DKV>
+constexpr int bwd_nwg() { return HD == 128 || (HD == 64 && DKV) ? 2 : (HD == 32 && !DKV) ? 4 : 3; }
+
+template <int HD, int NWG>
 struct BwdCfg {
   using A = AttnCfg<HD>;
-  // two resident [128 x HD] tiles (T0, T1), kBwdStages stages of the two streamed [64 x HD] tiles and of the streamed
+  // two resident [64 NWG x HD] tiles (T0, T1), kBwdStages stages of the two streamed [64 x HD] tiles and of the streamed
   // rows' lse2 / delta (dK/dV kernel only)
-  static constexpr int RES = A::template tile_bytes<128>();
+  static constexpr int RES = A::template tile_bytes<AttnWarps<NWG>::ROWS>();
   static constexpr int STR = A::template tile_bytes<kBwdStream>();
   static constexpr int T0 = 0, T1 = RES;
   static constexpr int S_OFF = 2 * RES;                 // stage st: tile a at S_OFF + st * 2 * STR, tile b at + STR
@@ -81,25 +87,27 @@ __global__ void __launch_bounds__(256) attn_delta_kernel(const __nv_bfloat16* __
 }
 
 // ---------------------------------------------------------------------------------------------
-// DKV = true : CTA = (128-key tile, sequence, head); resident K, V; streamed Q_i, dO_i.  Writes dK, dV.
-// DKV = false: CTA = (128-query tile, sequence, head); resident Q, dO; streamed K_j, V_j.  Writes dQ.
+// DKV = true : CTA = (64 NWG-key tile, sequence, head); resident K, V; streamed Q_i, dO_i.  Writes dK, dV.
+// DKV = false: CTA = (64 NWG-query tile, sequence, head); resident Q, dO; streamed K_j, V_j.  Writes dQ.
 // The two share the pipeline and the P / dS algebra; only the orientation of the score fragment differs: in the dK/dV
 // kernel the fragment's rows are keys and its columns queries (lse2 / delta are per column), in the dQ kernel the
 // reverse (lse2 / delta per row).
 // ---------------------------------------------------------------------------------------------
-template <int HD, bool DKV>
-__global__ void __launch_bounds__(kBwdThreads, 1)
+template <int HD, bool DKV, int NWG>
+__global__ void __launch_bounds__(AttnWarps<NWG>::THREADS, 1)
 attn_bwd_kernel(const __grid_constant__ CUtensorMap tmRes, const __grid_constant__ CUtensorMap tmStr,
                 const __grid_constant__ CUtensorMap tmDO, const AttnBwdParams p) {
-  using B = BwdCfg<HD>;
+  using B = BwdCfg<HD, NWG>;
+  using W = AttnWarps<NWG>;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
 
   const int seq = blockIdx.y, head = blockIdx.z;
   const int row_begin = p.cu_seqlens[seq];
   const int len = p.cu_seqlens[seq + 1] - row_begin;
-  const int t0 = blockIdx.x * 128;   // first resident row (key for DKV, query otherwise)
+  const int t0 = blockIdx.x * W::ROWS;   // first resident row (key for DKV, query otherwise)
   if (t0 >= len) return;
+  const int n_wg = attn_active_wgs<NWG>(len, t0);
   const int n_it = (len + kBwdStream - 1) / kBwdStream;
   const int HHD = p.H * HD;
 
@@ -111,14 +119,14 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmRes, const __grid_constant
   const uint32_t sStat = smem_u32(smem + B::STAT_OFF);
   const float* lse_h = p.lse2 + (long long)head * p.T + row_begin;
   const float* del_h = p.delta + (long long)head * p.T + row_begin;
-  const int wg = threadIdx.x >> 7;
+  const int wg = __shfl_sync(0xffffffffu, threadIdx.x >> 7, 0);   // warp-uniform to the compiler: no divergent wgmma paths
   const int lane = threadIdx.x & 31;
 
   if (threadIdx.x == 0) {
     mbar_init(bar_res, 1);
     for (int st = 0; st < kBwdStages; ++st) {
       mbar_init(full0 + 8 * st, DKV ? 32 : 1);   // dK/dV: every producer lane arrives after its lse2 / delta stores
-      mbar_init(empty0 + 8 * st, 8);             // one arrive per consumer warp
+      mbar_init(empty0 + 8 * st, 4 * n_wg);      // one arrive per active consumer warp
     }
     fence_mbar_init();
   }
@@ -127,16 +135,16 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmRes, const __grid_constant
   // resident: DKV -> T0 = K, T1 = V;  dQ -> T0 = Q, T1 = dO.   streamed: DKV -> a = Q_i, b = dO_i;  dQ -> a = K_j, b = V_j
   if (wg == 0) {
     // ------------------------------------------------------------------ producer (warp 0)
-    setmaxnreg_dec<40>();
+    setmaxnreg_dec<W::PRODUCER_REGS>();
     if (threadIdx.x < 32) {
       if (lane == 0) {
         mbar_expect_tx(bar_res, 2 * B::RES);
         if (DKV) {
-          attn_load_tile<HD, 128>(sT0, &tmRes, bar_res, HHD + head * HD, row_begin + t0);
-          attn_load_tile<HD, 128>(sT1, &tmRes, bar_res, 2 * HHD + head * HD, row_begin + t0);
+          attn_load_tile<HD, W::ROWS>(sT0, &tmRes, bar_res, HHD + head * HD, row_begin + t0);
+          attn_load_tile<HD, W::ROWS>(sT1, &tmRes, bar_res, 2 * HHD + head * HD, row_begin + t0);
         } else {
-          attn_load_tile<HD, 128>(sT0, &tmRes, bar_res, head * HD, row_begin + t0);
-          attn_load_tile<HD, 128>(sT1, &tmDO, bar_res, head * HD, row_begin + t0);
+          attn_load_tile<HD, W::ROWS>(sT0, &tmRes, bar_res, head * HD, row_begin + t0);
+          attn_load_tile<HD, W::ROWS>(sT1, &tmDO, bar_res, head * HD, row_begin + t0);
         }
       }
       for (int i = 0; i < n_it; ++i) {
@@ -171,8 +179,9 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmRes, const __grid_constant
   }
 
   // -------------------------------------------------------------------- consumers
-  setmaxnreg_inc<232>();
-  const int cw = wg - 1;   // which 64-row half of the resident tile
+  const int cw = wg - 1;   // which 64 rows of the resident tile
+  if (cw >= n_wg) return;
+  setmaxnreg_inc<W::CONSUMER_REGS>();
   const int r = cw * 64 + ((threadIdx.x >> 5) & 3) * 16 + (lane >> 2);   // first fragment row in the resident tile
   float acc0[HD / 2], acc1[HD / 2];   // DKV: dV, dK;  dQ: dQ (acc1 unused)
 #pragma unroll
@@ -197,11 +206,11 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmRes, const __grid_constant
     wgmma_fence();
 #pragma unroll
     for (int kk = 0; kk < HD / 16; ++kk)
-      wgmma_ss<kBwdStream, 0, 0>(x, attn_kmajor_desc<HD, 128>(sT0, cw * 64, kk), attn_kmajor_desc<HD, kBwdStream>(sa, 0, kk),
+      wgmma_ss<kBwdStream, 0, 0>(x, attn_kmajor_desc<HD, W::ROWS>(sT0, cw * 64, kk), attn_kmajor_desc<HD, kBwdStream>(sa, 0, kk),
                                  kk > 0);
 #pragma unroll
     for (int kk = 0; kk < HD / 16; ++kk)
-      wgmma_ss<kBwdStream, 0, 0>(y, attn_kmajor_desc<HD, 128>(sT1, cw * 64, kk), attn_kmajor_desc<HD, kBwdStream>(sb, 0, kk),
+      wgmma_ss<kBwdStream, 0, 0>(y, attn_kmajor_desc<HD, W::ROWS>(sT1, cw * 64, kk), attn_kmajor_desc<HD, kBwdStream>(sb, 0, kk),
                                  kk > 0);
     wgmma_commit();
     wgmma_wait<0>();
@@ -267,22 +276,27 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmRes, const __grid_constant
 template <int HD>
 static int launch_attn_bwd(const void* qkv, const void* out, const void* dout, const float* lse2, float* delta,
                            void* dqkv, const int* cu, int nseq, int max_len, int H, int T, float scale, cudaStream_t s) {
+  constexpr int NKV = bwd_nwg<HD, true>(), NQ = bwd_nwg<HD, false>();
   using C = AttnCfg<HD>;
-  using B = BwdCfg<HD>;
-  CUtensorMap tq128, tq64, tdo128, tdo64;
-  const uint64_t W = (uint64_t)3 * H * HD;
-  int rc = make_tmap_2d(&tq128, qkv, 0, W, T, W * 2, C::BOX_INNER, 128, C::TMAP_SWIZZLE);
+  using BKV = BwdCfg<HD, NKV>;
+  using BQ = BwdCfg<HD, NQ>;
+  using WKV = AttnWarps<NKV>;
+  using WQ = AttnWarps<NQ>;
+  // resident tiles: K, V (dK/dV kernel) and Q, dO (dQ kernel) in boxes of their kernel's resident rows
+  CUtensorMap tq_kv, tq_q, tdo_q, tq64, tdo64;
+  const uint64_t W = (uint64_t)3 * H * HD, WO = (uint64_t)H * HD;
+  int rc = make_tmap_2d(&tq_kv, qkv, 0, W, T, W * 2, C::BOX_INNER, WKV::ROWS, C::TMAP_SWIZZLE);
+  if (!rc) rc = make_tmap_2d(&tq_q, qkv, 0, W, T, W * 2, C::BOX_INNER, WQ::ROWS, C::TMAP_SWIZZLE);
   if (!rc) rc = make_tmap_2d(&tq64, qkv, 0, W, T, W * 2, C::BOX_INNER, kBwdStream, C::TMAP_SWIZZLE);
-  if (!rc) rc = make_tmap_2d(&tdo128, dout, 0, (uint64_t)H * HD, T, (uint64_t)H * HD * 2, C::BOX_INNER, 128, C::TMAP_SWIZZLE);
-  if (!rc) rc = make_tmap_2d(&tdo64, dout, 0, (uint64_t)H * HD, T, (uint64_t)H * HD * 2, C::BOX_INNER, kBwdStream,
-                             C::TMAP_SWIZZLE);
+  if (!rc) rc = make_tmap_2d(&tdo_q, dout, 0, WO, T, WO * 2, C::BOX_INNER, WQ::ROWS, C::TMAP_SWIZZLE);
+  if (!rc) rc = make_tmap_2d(&tdo64, dout, 0, WO, T, WO * 2, C::BOX_INNER, kBwdStream, C::TMAP_SWIZZLE);
   if (rc) return rc;
-  auto kdkv = attn_bwd_kernel<HD, true>;
-  auto kdq = attn_bwd_kernel<HD, false>;
+  auto kdkv = attn_bwd_kernel<HD, true, NKV>;
+  auto kdq = attn_bwd_kernel<HD, false, NQ>;
   static bool configured = false;
   if (!configured) {
-    VJ_CUDA(cudaFuncSetAttribute(kdkv, cudaFuncAttributeMaxDynamicSharedMemorySize, B::SMEM_BYTES));
-    VJ_CUDA(cudaFuncSetAttribute(kdq, cudaFuncAttributeMaxDynamicSharedMemorySize, B::SMEM_BYTES));
+    VJ_CUDA(cudaFuncSetAttribute(kdkv, cudaFuncAttributeMaxDynamicSharedMemorySize, BKV::SMEM_BYTES));
+    VJ_CUDA(cudaFuncSetAttribute(kdq, cudaFuncAttributeMaxDynamicSharedMemorySize, BQ::SMEM_BYTES));
     configured = true;
   }
   {
@@ -297,10 +311,9 @@ static int launch_attn_bwd(const void* qkv, const void* out, const void* dout, c
   AttnBwdParams p;
   p.cu_seqlens = cu; p.lse2 = lse2; p.delta = delta; p.dqkv = reinterpret_cast<__nv_bfloat16*>(dqkv);
   p.H = H; p.T = T; p.scale = scale; p.scale_log2 = scale * 1.4426950408889634f;
-  dim3 grid((max_len + 127) / 128, nseq, H);
-  kdkv<<<grid, kBwdThreads, B::SMEM_BYTES, s>>>(tq128, tq64, tdo64, p);
+  kdkv<<<dim3((max_len + WKV::ROWS - 1) / WKV::ROWS, nseq, H), WKV::THREADS, BKV::SMEM_BYTES, s>>>(tq_kv, tq64, tdo64, p);
   VJ_CUDA(cudaGetLastError());
-  kdq<<<grid, kBwdThreads, B::SMEM_BYTES, s>>>(tq128, tq64, tdo128, p);
+  kdq<<<dim3((max_len + WQ::ROWS - 1) / WQ::ROWS, nseq, H), WQ::THREADS, BQ::SMEM_BYTES, s>>>(tq_q, tq64, tdo_q, p);
   VJ_CUDA(cudaGetLastError());
   vj::count_launch(2);
   return 0;

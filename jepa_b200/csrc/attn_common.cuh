@@ -21,6 +21,25 @@ struct AttnCfg {
   static constexpr int tile_bytes() { return ROWS * HD * 2; }
 };
 
+// Warp-specialised attention CTA: one producer warpgroup and NWG consumer warpgroups of 64 resident rows each.
+// setmaxnreg only moves registers between the warps of a CTA, so the pool is what the launch allocated:
+// 65536 / threads rounded down to 8 per thread (168 at 384 threads, 128 at 512, 96 at 640).
+template <int NWG>
+struct AttnWarps {
+  static constexpr int THREADS = 128 * (NWG + 1);
+  static constexpr int ROWS = 64 * NWG;   // resident rows per CTA
+  static constexpr int PRODUCER_REGS = NWG == 2 ? 40 : NWG == 3 ? 32 : 24;
+  static constexpr int CONSUMER_REGS = NWG == 2 ? 232 : NWG == 3 ? 160 : 112;
+  static_assert(NWG >= 2 && NWG <= 4, "2..4 consumer warpgroups");
+  static_assert(128 * PRODUCER_REGS + 128 * NWG * CONSUMER_REGS <= (65536 / THREADS) / 8 * 8 * THREADS,
+                "setmaxnreg split exceeds the registers allocated at launch");
+};
+
+// Consumer warpgroups of a resident tile starting at row t0 that hold at least one of the sequence's len rows.  The
+// others never touch a barrier of the loop and exit after the set-up barrier.
+template <int NWG>
+VJ_DEVINL int attn_active_wgs(int len, int t0) { return min(NWG, (len - t0 + 63) / 64); }
+
 // K-major descriptor (reduction over HD) of k-step kk (16 elements) of a [ROWS x HD] tile, starting at row `row0`
 template <int HD, int ROWS>
 VJ_DEVINL uint64_t attn_kmajor_desc(uint32_t tile, int row0, int kk) {

@@ -8,18 +8,20 @@
 // layout the qkv GEMM epilogue writes), O bf16 [T, H*HD], lse2 fp32 [H, T] (log2 domain:
 // m*scale*log2e + log2(l)).  Sequences are row ranges [cu[s], cu[s+1]).
 //
-// One CTA = one 128-row query tile of one (sequence, head); K_j / V_j tiles of 128 keys stream through a 3-stage TMA ring.
-// Warp-specialised, three warpgroups (the FlashAttention-3 schedule):
-//   warpgroup 0   : TMA producer (one thread loads Q, then K_j / V_j into stage j % 3 once both consumers released it;
-//                   per-stage full (tx-count) and empty (one arrive per consumer warp) mbarriers)
-//   warpgroups 1-2: consumers, 64 query rows each.  S = Q K_j^T (wgmma, both operands in smem), online softmax on the
+// One CTA = one query tile of 64 * NWG rows of one (sequence, head); K_j / V_j tiles of 128 keys stream through a 3-stage
+// TMA ring.  Warp-specialised, NWG + 1 warpgroups (the FlashAttention-3 schedule):
+//   warpgroup 0   : TMA producer (one thread loads Q, then K_j / V_j into stage j % 3 once every active consumer released
+//                   it; per-stage full (tx-count) and empty (one arrive per active consumer warp) mbarriers)
+//   warpgroups 1..NWG: consumers, 64 query rows each.  S = Q K_j^T (wgmma, both operands in smem), online softmax on the
 //                   accumulator fragment in registers, O += P V_j with P as the register A operand (no shared-memory round
-//                   trip) and V_j read MN-major.
+//                   trip) and V_j read MN-major.  A consumer whose 64 rows all lie past the sequence's end exits at once.
 // Two overlaps keep the tensor cores busy while the exps run:
 //   - inside a warpgroup, S_j = Q K_j^T is issued together with O += P_{j-1} V_{j-1} (P_{j-1} held as bf16 fragments), so
 //     the softmax of S_j runs under P_{j-1} V_{j-1}; O is rescaled by alpha_j once that MMA has retired;
-//   - between the warpgroups, two named barriers make them take turns issuing (ping-pong), so one warpgroup's softmax runs
-//     under the other's MMAs.
+//   - between the warpgroups, a ring of named barriers makes them take turns issuing (round robin), so one warpgroup's
+//     softmax runs under the others' MMAs.
+// More consumer warpgroups per CTA put more independent softmax chains on each warp scheduler and share each K / V tile
+// among more query rows; NWG is chosen per head dim (fwd_nwg).
 // Only the ragged last KV tile of a sequence pays for the key mask.
 // The per-row arithmetic and its order over the KV tiles are those of a plain one-tile-at-a-time loop, so O and lse2 do
 // not depend on the schedule.
@@ -30,7 +32,6 @@
 
 namespace vj {
 
-constexpr int kFwdThreads = 384;
 constexpr int kFwdKV = 128;   // keys per tile
 constexpr int kFwdStages = 3;
 
@@ -43,34 +44,38 @@ struct AttnFwdParams {
   float scale_log2;
 };
 
+// Consumer warpgroups per CTA, measured per head dim (DESIGN section 6); hd 128's accumulators only fit two.
 template <int HD>
+constexpr int fwd_nwg() { return HD == 128 ? 2 : 3; }
+
+template <int HD, int NWG>
 struct FwdCfg {
   using A = AttnCfg<HD>;
-  static constexpr int TILE = A::template tile_bytes<128>();
+  using W = AttnWarps<NWG>;
+  static constexpr int TILE = A::template tile_bytes<kFwdKV>();
+  static constexpr int Q_TILE = A::template tile_bytes<W::ROWS>();
   static constexpr int Q_OFF = 0;
-  static constexpr int K_OFF = TILE;                          // kFwdStages stages
+  static constexpr int K_OFF = Q_TILE;                        // kFwdStages stages
   static constexpr int V_OFF = K_OFF + kFwdStages * TILE;     // kFwdStages stages
   static constexpr int BAR_OFF = V_OFF + kFwdStages * TILE;   // Q, full[stages], empty[stages]
   static constexpr int SMEM_BYTES = BAR_OFF + 8 * (1 + 2 * kFwdStages) + 1024;
   static_assert(SMEM_BYTES <= 232448, "attention forward shared memory budget exceeded");
 };
 
-// Ping-pong between the consumer warpgroups cw = 0, 1: named barrier 1 + cw opens cw's turn to issue MMAs.
-VJ_DEVINL void pingpong_wait_turn(int cw) { named_bar_sync(1 + cw, 256); }
-VJ_DEVINL void pingpong_pass_turn(int cw) { named_bar_arrive(2 - cw, 256); }
-
-template <int HD>
-__global__ void __launch_bounds__(kFwdThreads, 1)
-attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQKV, const AttnFwdParams p) {
-  using F = FwdCfg<HD>;
+template <int HD, int NWG>
+__global__ void __launch_bounds__(AttnWarps<NWG>::THREADS, 1)
+attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmKV, const AttnFwdParams p) {
+  using F = FwdCfg<HD, NWG>;
+  using W = AttnWarps<NWG>;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
 
   const int seq = blockIdx.y, head = blockIdx.z;
   const int row_begin = p.cu_seqlens[seq];
   const int len = p.cu_seqlens[seq + 1] - row_begin;
-  const int q0 = blockIdx.x * 128;
+  const int q0 = blockIdx.x * W::ROWS;
   if (q0 >= len) return;
+  const int n_wg = attn_active_wgs<NWG>(len, q0);
   const int n_kv = (len + kFwdKV - 1) / kFwdKV;
 
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + F::BAR_OFF);
@@ -79,40 +84,42 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQKV, const AttnFwdParams p
   const uint32_t empty0 = smem_u32(bars + 1 + kFwdStages);
   const uint32_t sQ = smem_u32(smem + F::Q_OFF), sK = smem_u32(smem + F::K_OFF), sV = smem_u32(smem + F::V_OFF);
   const int HHD = p.H * HD;
-  const int wg = threadIdx.x >> 7;
+  const int wg = __shfl_sync(0xffffffffu, threadIdx.x >> 7, 0);   // warp-uniform to the compiler: no divergent wgmma paths
 
   if (threadIdx.x == 0) {
     mbar_init(bar_q, 1);
     for (int st = 0; st < kFwdStages; ++st) {
       mbar_init(full0 + 8 * st, 1);
-      mbar_init(empty0 + 8 * st, 8);   // one arrive per consumer warp
+      mbar_init(empty0 + 8 * st, 4 * n_wg);   // one arrive per active consumer warp
     }
     fence_mbar_init();
-    tma_prefetch_desc(&tmQKV);
+    tma_prefetch_desc(&tmQ);
+    tma_prefetch_desc(&tmKV);
   }
   __syncthreads();
 
   if (wg == 0) {
     // ------------------------------------------------------------------ TMA producer
-    setmaxnreg_dec<40>();
+    setmaxnreg_dec<W::PRODUCER_REGS>();
     if (threadIdx.x == 0) {
-      mbar_expect_tx(bar_q, F::TILE);
-      attn_load_tile<HD, 128>(sQ, &tmQKV, bar_q, head * HD, row_begin + q0);
+      mbar_expect_tx(bar_q, F::Q_TILE);
+      attn_load_tile<HD, W::ROWS>(sQ, &tmQ, bar_q, head * HD, row_begin + q0);
       for (int j = 0; j < n_kv; ++j) {
         const int st = j % kFwdStages;
         mbar_wait(empty0 + 8 * st, ((j / kFwdStages) & 1) ^ 1);
         const uint32_t fb = full0 + 8 * st;
         mbar_expect_tx(fb, 2 * F::TILE);
-        attn_load_tile<HD, 128>(sK + st * F::TILE, &tmQKV, fb, HHD + head * HD, row_begin + j * kFwdKV);
-        attn_load_tile<HD, 128>(sV + st * F::TILE, &tmQKV, fb, 2 * HHD + head * HD, row_begin + j * kFwdKV);
+        attn_load_tile<HD, kFwdKV>(sK + st * F::TILE, &tmKV, fb, HHD + head * HD, row_begin + j * kFwdKV);
+        attn_load_tile<HD, kFwdKV>(sV + st * F::TILE, &tmKV, fb, 2 * HHD + head * HD, row_begin + j * kFwdKV);
       }
     }
     return;
   }
 
   // -------------------------------------------------------------------- consumers
-  setmaxnreg_inc<232>();
-  const int cw = wg - 1;   // which 64-row half of the query tile
+  const int cw = wg - 1;   // which 64 rows of the query tile
+  if (cw >= n_wg) return;
+  setmaxnreg_inc<W::CONSUMER_REGS>();
   const int lane = threadIdx.x & 31;
   const int r = cw * 64 + ((threadIdx.x >> 5) & 3) * 16 + (lane >> 2);   // this thread's first row in the tile (+8: second)
   float o[HD / 2];
@@ -121,18 +128,25 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQKV, const AttnFwdParams p
   float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
   float s[kFwdKV / 2];              // S_j, then P_j (fp32)
   uint32_t pf[kFwdKV / 16][4];      // P_{j-1} as bf16 A fragments, read by the in-flight P_{j-1} V_{j-1}
-  if (cw == 1) pingpong_pass_turn(cw);   // warpgroup 0 issues first
+  // Round robin among the n_wg active warpgroups: named barrier 1 + cw opens cw's turn to issue MMAs.
+  auto wait_turn = [&]() {
+    if (n_wg > 1) named_bar_sync(1 + cw, 256);
+  };
+  auto pass_turn = [&]() {
+    if (n_wg > 1) named_bar_arrive(cw + 1 == n_wg ? 1 : 2 + cw, 256);
+  };
+  if (cw == n_wg - 1) pass_turn();   // warpgroup 0 issues first
 
   auto issue_s = [&](int st) {
 #pragma unroll
     for (int kk = 0; kk < HD / 16; ++kk)
-      wgmma_ss<kFwdKV, 0, 0>(s, attn_kmajor_desc<HD, 128>(sQ, cw * 64, kk),
-                             attn_kmajor_desc<HD, 128>(sK + st * F::TILE, 0, kk), kk > 0);
+      wgmma_ss<kFwdKV, 0, 0>(s, attn_kmajor_desc<HD, W::ROWS>(sQ, cw * 64, kk),
+                             attn_kmajor_desc<HD, kFwdKV>(sK + st * F::TILE, 0, kk), kk > 0);
     wgmma_commit();
   };
   auto issue_pv = [&](int st) {
 #pragma unroll
-    for (int kk = 0; kk < kFwdKV / 16; ++kk) wgmma_rs<HD, 1>(o, pf[kk], attn_mnmajor_desc<HD, 128>(sV + st * F::TILE, kk), 1);
+    for (int kk = 0; kk < kFwdKV / 16; ++kk) wgmma_rs<HD, 1>(o, pf[kk], attn_mnmajor_desc<HD, kFwdKV>(sV + st * F::TILE, kk), 1);
     wgmma_commit();
   };
   auto release = [&](int st) {
@@ -188,11 +202,11 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQKV, const AttnFwdParams p
   mbar_wait(bar_q, 0);
   // tile 0: S_0 alone
   float alpha[2];
-  pingpong_wait_turn(cw);
+  wait_turn();
   mbar_wait(full0, 0);
   wgmma_fence();
   issue_s(0);
-  pingpong_pass_turn(cw);
+  pass_turn();
   wgmma_wait<0>();
   wgmma_fence_regs(s);
   softmax(0, alpha);
@@ -201,13 +215,13 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQKV, const AttnFwdParams p
   // tile j: S_j together with P_{j-1} V_{j-1}
   for (int j = 1; j < n_kv; ++j) {
     const int st = j % kFwdStages, st_prev = (j - 1) % kFwdStages;
-    pingpong_wait_turn(cw);
+    wait_turn();
     mbar_wait(full0 + 8 * st, (j / kFwdStages) & 1);
     wgmma_fence_regs(o);
     wgmma_fence();
     issue_s(st);
     issue_pv(st_prev);
-    pingpong_pass_turn(cw);
+    pass_turn();
     wgmma_wait<1>();   // S_j is ready, P_{j-1} V_{j-1} may still run
     wgmma_fence_regs(s);
     softmax(j, alpha);
@@ -219,15 +233,15 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQKV, const AttnFwdParams p
     pack_p();
   }
   // last P V
-  pingpong_wait_turn(cw);
+  wait_turn();
   wgmma_fence_regs(o);
   wgmma_fence();
   issue_pv((n_kv - 1) % kFwdStages);
-  pingpong_pass_turn(cw);
+  pass_turn();
   wgmma_wait<0>();
   wgmma_fence_regs(o);
   wgmma_fence_regs(pf);
-  if (cw == 0) pingpong_wait_turn(cw);   // takes warpgroup 1's last pass, so both barriers end balanced
+  if (cw == 0) wait_turn();   // takes the last warpgroup's last pass, so every turn barrier ends balanced
 
   // ---- epilogue: O / l -> bf16, lse2 (log2 domain)
   float inv[2];
@@ -249,13 +263,16 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQKV, const AttnFwdParams p
 template <int HD>
 static int launch_attn_fwd(const void* qkv, void* out, float* lse2, const int* cu, int nseq, int max_len, int H, int T,
                            float scale, cudaStream_t s) {
+  constexpr int NWG = fwd_nwg<HD>();
   using C = AttnCfg<HD>;
-  using F = FwdCfg<HD>;
-  CUtensorMap tm;
-  int rc = make_tmap_2d(&tm, qkv, 0, (uint64_t)3 * H * HD, T, (uint64_t)3 * H * HD * 2, C::BOX_INNER, 128,
-                        C::TMAP_SWIZZLE);
+  using F = FwdCfg<HD, NWG>;
+  using W = AttnWarps<NWG>;
+  const uint64_t width = (uint64_t)3 * H * HD;
+  CUtensorMap tmq, tmkv;
+  int rc = make_tmap_2d(&tmq, qkv, 0, width, T, width * 2, C::BOX_INNER, W::ROWS, C::TMAP_SWIZZLE);
+  if (!rc) rc = make_tmap_2d(&tmkv, qkv, 0, width, T, width * 2, C::BOX_INNER, kFwdKV, C::TMAP_SWIZZLE);
   if (rc) return rc;
-  auto kern = attn_fwd_kernel<HD>;
+  auto kern = attn_fwd_kernel<HD, NWG>;
   static bool configured = false;
   if (!configured) {
     VJ_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, F::SMEM_BYTES));
@@ -265,8 +282,8 @@ static int launch_attn_fwd(const void* qkv, void* out, float* lse2, const int* c
   p.cu_seqlens = cu; p.out = reinterpret_cast<__nv_bfloat16*>(out); p.lse2 = lse2;
   p.H = H; p.T = T; p.ld_out = (long long)H * HD;
   p.scale_log2 = scale * 1.4426950408889634f;
-  dim3 grid((max_len + 127) / 128, nseq, H);
-  kern<<<grid, kFwdThreads, F::SMEM_BYTES, s>>>(tm, p);
+  dim3 grid((max_len + W::ROWS - 1) / W::ROWS, nseq, H);
+  kern<<<grid, W::THREADS, F::SMEM_BYTES, s>>>(tmq, tmkv, p);
   VJ_CUDA(cudaGetLastError());
   vj::count_launch(1);
   return 0;
