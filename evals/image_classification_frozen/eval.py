@@ -5,8 +5,10 @@ eval.py:63-521): a video encoder from pre-training sees each image repeated `fra
 reference :451-456), and the attentive probe trains on its tokens with one classifier call per step.  The optimizer,
 checkpoint and encoder-loading helpers are the video evaluation's (the reference has identical copies).
 
-The reference autocasts the loop to fp16 (eval.py:284).  The kernels here compute bf16 x bf16 -> fp32 whatever autocast
-says, so there is no autocast region: `use_bfloat16` selects the GradScaler, as it does in the reference.
+The reference autocasts the loop to fp16 (eval.py:284).  This loop opens no autocast region, so encoder and probe compute
+bf16 x bf16 -> fp32, and `use_bfloat16` selects the GradScaler, as it does in the reference.  (Inside a caller's
+autocast(float16) the encoder would run its fp16 kernels and return fp32 features; the probe computes in bf16 either
+way.)
 """
 import os
 
@@ -172,7 +174,7 @@ def run_one_epoch(device, training, encoder, classifier, scaler, optimizer, sche
             scheduler.step()
             wd_scheduler.step()
 
-        # (no autocast: the kernels compute bf16 x bf16 -> fp32 regardless; see the module docstring)
+        # (no autocast region: encoder and probe compute bf16 x bf16 -> fp32; see the module docstring)
         if isinstance(data[0], list):       # uint8 image tickets: the transform's pixel work runs on the GPU
             imgs = data_loader.dataset.transform.batch(data[0], device)
         else:

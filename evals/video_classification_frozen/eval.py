@@ -9,8 +9,10 @@ eval.py:67-561), with every step on the sm_90a kernels of jepa_b200:
   DistributedDataParallel                           -> one averaging all-reduce of the probe's flat gradient per backward
   validation views (uint8 frames)                   -> vj_clip_views (EvalVideoTransform / VideoTransform eval path)
 
-The reference autocasts the loop to fp16 (eval.py:323).  The kernels here compute bf16 x bf16 -> fp32 whatever autocast
-says, so there is no autocast region: `use_bfloat16` selects the GradScaler, as it does in the reference.
+The reference autocasts the loop to fp16 (eval.py:323).  This loop opens no autocast region, so encoder and probe compute
+bf16 x bf16 -> fp32, and `use_bfloat16` selects the GradScaler, as it does in the reference.  (Inside a caller's
+autocast(float16) the encoder would run its fp16 kernels and return fp32 features; the probe computes in bf16 either
+way.)
 """
 import os
 
@@ -232,7 +234,7 @@ def run_one_epoch(device, training, encoder, classifier, scaler, optimizer, sche
             scheduler.step()
             wd_scheduler.step()
 
-        # (no autocast: the kernels compute bf16 x bf16 -> fp32 regardless; see the module docstring)
+        # (no autocast region: encoder and probe compute bf16 x bf16 -> fp32; see the module docstring)
         clips = load_clips(data, device, data_loader)
         clip_indices = [d.to(device, non_blocking=True) for d in data[2]]
         labels = data[1].to(device)

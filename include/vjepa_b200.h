@@ -60,6 +60,16 @@ int vj_gemm(const void* A, long long lda, int a_mn, const void* B, long long ldb
             int epi, const void* aux, long long ldaux, int aux_f32, const int* aux_rowmap,
             int aux_period, void* aux_out, long long ldauxout, int split_k, int accumulate,
             void* stream);
+/* vj_gemm with fp16 operands: A, B and every 16-bit D / aux / aux_out are fp16 (d_f32 = 0 / aux_f32 = 0), fp32 D and
+ * fp32 aux as above.  Frozen evaluation under torch.cuda.amp.autocast(dtype=torch.float16)
+ * (evals/video_classification_frozen/eval.py:323, evals/image_classification_frozen/eval.py:284), where F.linear and
+ * the Conv3d of the patch embedding run in fp16.  Instantiated: forward (0,0) with NONE / GELU / GELU_GRAD / ADD (fp16
+ * or row-mapped / periodic fp32 aux), dgrad (0,1) plain and MUL, wgrad (1,1) into fp32. */
+int vj_gemm_f16(const void* A, long long lda, int a_mn, const void* B, long long ldb, int b_mn,
+                void* D, long long ldd, int d_f32, int M, int N, int K, const float* bias, float alpha,
+                int epi, const void* aux, long long ldaux, int aux_f32, const int* aux_rowmap,
+                int aux_period, void* aux_out, long long ldauxout, int split_k, int accumulate,
+                void* stream);
 
 /* Dense var-len flash attention forward (wgmma).  qkv bf16 [T, 3*H*HD] (q|k|v thirds, head-major),
  * out bf16 [T, H*HD], lse2 fp32 [H, T] (log2 domain).  Sequences are the row ranges
@@ -68,6 +78,10 @@ int vj_gemm(const void* A, long long lda, int a_mn, const void* B, long long ldb
  * Replaces F.scaled_dot_product_attention, src/models/utils/modules.py:66-69. */
 int vj_attn_fwd(const void* qkv, void* out, float* lse2, const int* cu_seqlens, int nseq, int max_len,
                 int H, int HD, int T, float scale, void* stream);
+/* vj_attn_fwd with fp16 qkv and out (P rounded to fp16 for P V): the SDPA of modules.py:66-69 under the evals'
+ * autocast(float16) (evals/video_classification_frozen/eval.py:323). */
+int vj_attn_fwd_f16(const void* qkv, void* out, float* lse2, const int* cu_seqlens, int nseq, int max_len,
+                    int H, int HD, int T, float scale, void* stream);
 
 /* Backward of the above: dqkv bf16 [T, 3*H*HD] from dout bf16 [T, H*HD]; delta_ws fp32 [H*T] scratch.
  * dq_acc_ws: unused (may be NULL); kept so callers built against earlier versions of this header still link.
@@ -77,7 +91,9 @@ int vj_attn_bwd(const void* qkv, const void* out, const void* dout, const float*
                 float scale, void* stream);
 
 /* LayerNorm over the last dim, one warp per row.  x bf16|fp32 [T,D] -> y bf16|fp32; mean/rstd fp32 [T]
- * (nullable) are saved for the backward.  nn.LayerNorm(eps=1e-6) at modules.py:115,119,
+ * (nullable) are saved for the backward.  x_f32 / y_f32 = 2: fp16, paired with fp16 or fp32 (LayerNorm under the
+ * evals' autocast(float16), evals/video_classification_frozen/eval.py:323: fp16 in, fp32 out, or fused with the
+ * following Linear's cast to fp16).  nn.LayerNorm(eps=1e-6) at modules.py:115,119,
  * vision_transformer.py:192-193, predictor.py:233. */
 int vj_layernorm_fwd(const void* x, int x_f32, void* y, int y_f32, const float* gamma, const float* beta,
                      float* mean, float* rstd, int T, int D, float eps, void* stream);
@@ -97,6 +113,10 @@ int vj_colsum(const void* in, int in_f32, float* out, long long T, int N, long l
  * PatchEmbed3D, src/models/utils/patch_embed.py:47-57 (+ apply_masks, vision_transformer.py:178-180). */
 int vj_im2col_tubelets(const float* clips, void* patches, const long long* idx, int B, int C, int T, int H,
                        int W, int tubelet, int patch, int K, void* stream);
+/* The same with fp16 patches: the Conv3d input cast of PatchEmbed3D under the evals' autocast(float16)
+ * (evals/video_classification_frozen/eval.py:323). */
+int vj_im2col_tubelets_f16(const float* clips, void* patches, const long long* idx, int B, int C, int T, int H,
+                           int W, int tubelet, int patch, int K, void* stream);
 
 /* Positional-embedding resampling for off-size encoder inputs (interpolate_pos_encoding,
  * src/models/vision_transformer.py:197-246): fp32 in [Nt,Nh,Nw,D] -> fp32 out [T,H,W,D], bit-exact with torch's CPU
@@ -173,8 +193,12 @@ int vj_cross_attn_bwd(const void* q, const void* kv, const void* out, const void
 /* dst bf16[n] = src fp32[n]: the per-step bf16 shadow of the fp32 master weights (what autocast's
  * weight cast does for every F.linear under torch.cuda.amp.autocast, app/vjepa/train.py:453). */
 int vj_cast_f32_bf16(const float* src, void* dst, long long n, void* stream);
+/* dst fp16[n] = src fp32[n]: the fp16 shadow, autocast(float16)'s weight cast in the eval loops
+ * (evals/video_classification_frozen/eval.py:323, evals/image_classification_frozen/eval.py:284). */
+int vj_cast_f32_f16(const float* src, void* dst, long long n, void* stream);
 /* Tensors viewed as [outer, G, hd, inner] <-> [outer, G, hdp, inner]: zero-pad heads (unpad_add=0) or
- * accumulate the padded fp32 gradient back into the unpadded one (unpad_add=1).  Predictor heads are
+ * accumulate the padded fp32 gradient back into the unpadded one (unpad_add=1).  dst_f32 = 2: an fp16 destination
+ * from an fp32 source (head-padded weights of an fp16 forward, ViT-H's hd 80 -> 128).  Predictor heads are
  * hd = 384/16 = 24 (app/vjepa/utils.py:119) and run as 32-wide wgmma tiles. */
 int vj_head_pad(const void* src, int src_f32, void* dst, int dst_f32, long long outer, int G, int hd, int hdp,
                 long long inner, int unpad_add, void* stream);

@@ -24,13 +24,16 @@ SIGNATURES = {
     "vj_image_views": (I, [P, P, P, P, P, I, I, I, P, P, P]),
     "vj_image_augment": (I, [P, P, P, P, P, P, P, P, P, P, I, P, P, I, I, I, P, P, P, P]),
     "vj_gemm": (I, [P, L, I, P, L, I, P, L, I, I, I, I, P, F, I, P, L, I, P, I, P, L, I, I, P]),
+    "vj_gemm_f16": (I, [P, L, I, P, L, I, P, L, I, I, I, I, P, F, I, P, L, I, P, I, P, L, I, I, P]),
     "vj_attn_fwd": (I, [P, P, P, P, I, I, I, I, I, F, P]),
+    "vj_attn_fwd_f16": (I, [P, P, P, P, I, I, I, I, I, F, P]),
     "vj_attn_bwd": (I, [P, P, P, P, P, P, P, P, I, I, I, I, I, F, P]),
     "vj_layernorm_fwd": (I, [P, I, P, I, P, P, P, P, I, I, F, P]),
     "vj_layernorm_bwd_workspace": (Z, [I, I]),
     "vj_layernorm_bwd": (I, [P, P, I, P, P, P, P, P, P, P, P, Z, I, I, P]),
     "vj_colsum": (I, [P, I, P, L, I, L, I, I, I, P]),
     "vj_im2col_tubelets": (I, [P, P, P, I, I, I, I, I, I, I, I, P]),
+    "vj_im2col_tubelets_f16": (I, [P, P, P, I, I, I, I, I, I, I, I, P]),
     "vj_pos_interp": (I, [P, P, I, I, I, I, I, I, I, c_double, c_double, c_double, I, P]),
     "vj_gather_rows": (I, [P, P, P, I, I, I, I, P]),
     "vj_scatter_rows_add": (I, [P, P, P, I, I, I, I, I, P]),
@@ -49,6 +52,7 @@ SIGNATURES = {
     "vj_cross_attn_bwd": (I, [P, P, P, P, P, P, P, P, Z, I, I, I, I, I, F, P]),
     "vj_token_std_bwd": (I, [P, P, P, F, P, I, I, I, F, F, P]),
     "vj_cast_f32_bf16": (I, [P, P, L, P]),
+    "vj_cast_f32_f16": (I, [P, P, L, P]),
     "vj_head_pad": (I, [P, I, P, I, L, I, I, I, L, I, P]),
     "vj_ema_update": (I, [P, P, L, F, F, P]),
     "vj_adamw_step": (I, [P, P, P, P, L, F, F, F, F, F, I, P, P, P]),

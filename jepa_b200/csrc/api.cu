@@ -131,7 +131,11 @@ static int encode_tmap_2d(CUtensorMap* out, const void* ptr, int dtype, uint64_t
                           : swizzle == 2 ? CU_TENSOR_MAP_SWIZZLE_64B
                           : swizzle == 1 ? CU_TENSOR_MAP_SWIZZLE_32B
                                          : CU_TENSOR_MAP_SWIZZLE_NONE;
-  CUresult r = enc(out, dtype == 1 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2,
+  CUresult r = enc(out,
+                   dtype == 1   ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32
+                   : dtype == 2 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT16
+                                : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16,
+                   2,
                    const_cast<void*>(ptr), gdim, gstride, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, sw,
                    CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS) {

@@ -266,10 +266,10 @@ attn_bwd_kernel(const __grid_constant__ CUtensorMap tmRes, const __grid_constant
 
   __nv_bfloat16* rows = p.dqkv + (long long)(row_begin + t0) * 3 * HHD + head * HD;
   if (DKV) {
-    store_frag_bf16<HD>(acc1, p.scale, rows + HHD, 3LL * HHD, r, len - t0);       // dK
-    store_frag_bf16<HD>(acc0, 1.0f, rows + 2 * HHD, 3LL * HHD, r, len - t0);      // dV
+    store_frag<HD>(acc1, p.scale, rows + HHD, 3LL * HHD, r, len - t0);       // dK
+    store_frag<HD>(acc0, 1.0f, rows + 2 * HHD, 3LL * HHD, r, len - t0);      // dV
   } else {
-    store_frag_bf16<HD>(acc0, p.scale, rows, 3LL * HHD, r, len - t0);             // dQ
+    store_frag<HD>(acc0, p.scale, rows, 3LL * HHD, r, len - t0);             // dQ
   }
 }
 

@@ -64,13 +64,14 @@ VJ_DEVINL void attn_load_tile(uint32_t dst, const CUtensorMap* m, uint32_t bar, 
 }
 
 // m64k16 A fragment (registers) of k-step kk from an m64nN fp32 accumulator fragment of the same rows: the accumulator's
-// column pairs 16kk..16kk+15 are exactly the A operand's k pairs, so P / dS never touch shared memory.
-template <int R>
+// column pairs 16kk..16kk+15 are exactly the A operand's k pairs, so P / dS never touch shared memory.  T: the A
+// operand's element type (fp16: cvt.rn.f16x2.f32).
+template <typename T = __nv_bfloat16, int R>
 VJ_DEVINL void acc_to_afrag(const float (&d)[R], int kk, uint32_t (&a)[4]) {
-  a[0] = pack_bf16x2(d[8 * kk + 0], d[8 * kk + 1]);
-  a[1] = pack_bf16x2(d[8 * kk + 2], d[8 * kk + 3]);
-  a[2] = pack_bf16x2(d[8 * kk + 4], d[8 * kk + 5]);
-  a[3] = pack_bf16x2(d[8 * kk + 6], d[8 * kk + 7]);
+  a[0] = Elt<T>::pack(d[8 * kk + 0], d[8 * kk + 1]);
+  a[1] = Elt<T>::pack(d[8 * kk + 2], d[8 * kk + 3]);
+  a[2] = Elt<T>::pack(d[8 * kk + 4], d[8 * kk + 5]);
+  a[3] = Elt<T>::pack(d[8 * kk + 6], d[8 * kk + 7]);
 }
 
 VJ_DEVINL float quad_max(float v) {
@@ -82,10 +83,10 @@ VJ_DEVINL float quad_sum(float v) {
   return v + __shfl_xor_sync(0xffffffffu, v, 2);
 }
 
-// Stores an m64nHD fp32 accumulator fragment (times `mul`) as bf16 rows: thread holds rows r and r + 8 of the
-// warpgroup's 64, column pairs 8j + 2(lane % 4).  Rows at or beyond `rows_valid` are skipped.
-template <int HD>
-VJ_DEVINL void store_frag_bf16(const float (&d)[HD / 2], float mul, __nv_bfloat16* base, long long ld, int r, int rows_valid) {
+// Stores an m64nHD fp32 accumulator fragment (times `mul`) as T (bf16 or fp16) rows: thread holds rows r and r + 8 of
+// the warpgroup's 64, column pairs 8j + 2(lane % 4).  Rows at or beyond `rows_valid` are skipped.
+template <int HD, typename T = __nv_bfloat16>
+VJ_DEVINL void store_frag(const float (&d)[HD / 2], float mul, T* base, long long ld, int r, int rows_valid) {
   const int lane = threadIdx.x & 31;
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
@@ -94,7 +95,7 @@ VJ_DEVINL void store_frag_bf16(const float (&d)[HD / 2], float mul, __nv_bfloat1
 #pragma unroll
     for (int j = 0; j < HD / 8; ++j)
       *reinterpret_cast<uint32_t*>(base + (long long)row * ld + 8 * j + 2 * (lane & 3)) =
-          pack_bf16x2(d[4 * j + 2 * h] * mul, d[4 * j + 2 * h + 1] * mul);
+          Elt<T>::pack(d[4 * j + 2 * h] * mul, d[4 * j + 2 * h + 1] * mul);
   }
 }
 

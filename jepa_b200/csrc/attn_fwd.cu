@@ -4,9 +4,10 @@
 // argument there is ignored - "masked attention" is attention over the gathered token subset,
 // so every sequence is dense and only its length varies).
 //
-// Layout: qkv bf16 [T, 3*H*HD] (row = token, q|k|v packed, head-major inside each third - the
-// layout the qkv GEMM epilogue writes), O bf16 [T, H*HD], lse2 fp32 [H, T] (log2 domain:
-// m*scale*log2e + log2(l)).  Sequences are row ranges [cu[s], cu[s+1]).
+// Layout: qkv T [T, 3*H*HD] (row = token, q|k|v packed, head-major inside each third - the
+// layout the qkv GEMM epilogue writes), O T [T, H*HD], lse2 fp32 [H, T] (log2 domain:
+// m*scale*log2e + log2(l)).  Sequences are row ranges [cu[s], cu[s+1]).  T = bf16 (vj_attn_fwd) or fp16 (vj_attn_fwd_f16,
+// frozen evaluation under autocast(float16)); the schedule and the arithmetic are the same, P is packed to T.
 //
 // One CTA = one query tile of 64 * NWG rows of one (sequence, head); K_j / V_j tiles of 128 keys stream through a 3-stage
 // TMA ring.  Warp-specialised, NWG + 1 warpgroups (the FlashAttention-3 schedule):
@@ -37,7 +38,7 @@ constexpr int kFwdStages = 3;
 
 struct AttnFwdParams {
   const int* cu_seqlens;
-  __nv_bfloat16* out;
+  void* out;
   float* lse2;
   int H, T;
   long long ld_out;
@@ -62,7 +63,7 @@ struct FwdCfg {
   static_assert(SMEM_BYTES <= 232448, "attention forward shared memory budget exceeded");
 };
 
-template <int HD, int NWG>
+template <typename T, int HD, int NWG>
 __global__ void __launch_bounds__(AttnWarps<NWG>::THREADS, 1)
 attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmKV, const AttnFwdParams p) {
   using F = FwdCfg<HD, NWG>;
@@ -127,7 +128,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
   for (int i = 0; i < HD / 2; ++i) o[i] = 0.f;
   float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};
   float s[kFwdKV / 2];              // S_j, then P_j (fp32)
-  uint32_t pf[kFwdKV / 16][4];      // P_{j-1} as bf16 A fragments, read by the in-flight P_{j-1} V_{j-1}
+  uint32_t pf[kFwdKV / 16][4];      // P_{j-1} as T A fragments, read by the in-flight P_{j-1} V_{j-1}
   // Round robin among the n_wg active warpgroups: named barrier 1 + cw opens cw's turn to issue MMAs.
   auto wait_turn = [&]() {
     if (n_wg > 1) named_bar_sync(1 + cw, 256);
@@ -140,13 +141,13 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
   auto issue_s = [&](int st) {
 #pragma unroll
     for (int kk = 0; kk < HD / 16; ++kk)
-      wgmma_ss<kFwdKV, 0, 0>(s, attn_kmajor_desc<HD, W::ROWS>(sQ, cw * 64, kk),
+      wgmma_ss<kFwdKV, 0, 0, T>(s, attn_kmajor_desc<HD, W::ROWS>(sQ, cw * 64, kk),
                              attn_kmajor_desc<HD, kFwdKV>(sK + st * F::TILE, 0, kk), kk > 0);
     wgmma_commit();
   };
   auto issue_pv = [&](int st) {
 #pragma unroll
-    for (int kk = 0; kk < kFwdKV / 16; ++kk) wgmma_rs<HD, 1>(o, pf[kk], attn_mnmajor_desc<HD, kFwdKV>(sV + st * F::TILE, kk), 1);
+    for (int kk = 0; kk < kFwdKV / 16; ++kk) wgmma_rs<HD, 1, T>(o, pf[kk], attn_mnmajor_desc<HD, kFwdKV>(sV + st * F::TILE, kk), 1);
     wgmma_commit();
   };
   auto release = [&](int st) {
@@ -196,7 +197,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
   };
   auto pack_p = [&]() {
 #pragma unroll
-    for (int kk = 0; kk < kFwdKV / 16; ++kk) acc_to_afrag(s, kk, pf[kk]);
+    for (int kk = 0; kk < kFwdKV / 16; ++kk) acc_to_afrag<T>(s, kk, pf[kk]);
   };
 
   mbar_wait(bar_q, 0);
@@ -243,7 +244,7 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
   wgmma_fence_regs(pf);
   if (cw == 0) wait_turn();   // takes the last warpgroup's last pass, so every turn barrier ends balanced
 
-  // ---- epilogue: O / l -> bf16, lse2 (log2 domain)
+  // ---- epilogue: O / l -> T, lse2 (log2 domain)
   float inv[2];
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
@@ -257,11 +258,12 @@ attn_fwd_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__
     o[4 * c + 0] *= inv[0]; o[4 * c + 1] *= inv[0];
     o[4 * c + 2] *= inv[1]; o[4 * c + 3] *= inv[1];
   }
-  store_frag_bf16<HD>(o, 1.0f, p.out + (long long)(row_begin + q0) * p.ld_out + head * HD, p.ld_out, r, len - q0);
+  store_frag<HD>(o, 1.0f, reinterpret_cast<T*>(p.out) + (long long)(row_begin + q0) * p.ld_out + head * HD, p.ld_out, r,
+                      len - q0);
 }
 
-template <int HD>
-static int launch_attn_fwd(const void* qkv, void* out, float* lse2, const int* cu, int nseq, int max_len, int H, int T,
+template <typename T, int HD>
+static int launch_attn_fwd(const void* qkv, void* out, float* lse2, const int* cu, int nseq, int max_len, int H, int T_,
                            float scale, cudaStream_t s) {
   constexpr int NWG = fwd_nwg<HD>();
   using C = AttnCfg<HD>;
@@ -269,18 +271,18 @@ static int launch_attn_fwd(const void* qkv, void* out, float* lse2, const int* c
   using W = AttnWarps<NWG>;
   const uint64_t width = (uint64_t)3 * H * HD;
   CUtensorMap tmq, tmkv;
-  int rc = make_tmap_2d(&tmq, qkv, 0, width, T, width * 2, C::BOX_INNER, W::ROWS, C::TMAP_SWIZZLE);
-  if (!rc) rc = make_tmap_2d(&tmkv, qkv, 0, width, T, width * 2, C::BOX_INNER, kFwdKV, C::TMAP_SWIZZLE);
+  int rc = make_tmap_2d(&tmq, qkv, Elt<T>::kTmap, width, T_, width * 2, C::BOX_INNER, W::ROWS, C::TMAP_SWIZZLE);
+  if (!rc) rc = make_tmap_2d(&tmkv, qkv, Elt<T>::kTmap, width, T_, width * 2, C::BOX_INNER, kFwdKV, C::TMAP_SWIZZLE);
   if (rc) return rc;
-  auto kern = attn_fwd_kernel<HD, NWG>;
+  auto kern = attn_fwd_kernel<T, HD, NWG>;
   static bool configured = false;
   if (!configured) {
     VJ_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, F::SMEM_BYTES));
     configured = true;
   }
   AttnFwdParams p;
-  p.cu_seqlens = cu; p.out = reinterpret_cast<__nv_bfloat16*>(out); p.lse2 = lse2;
-  p.H = H; p.T = T; p.ld_out = (long long)H * HD;
+  p.cu_seqlens = cu; p.out = out; p.lse2 = lse2;
+  p.H = H; p.T = T_; p.ld_out = (long long)H * HD;
   p.scale_log2 = scale * 1.4426950408889634f;
   dim3 grid((max_len + W::ROWS - 1) / W::ROWS, nseq, H);
   kern<<<grid, W::THREADS, F::SMEM_BYTES, s>>>(tmq, tmkv, p);
@@ -289,20 +291,31 @@ static int launch_attn_fwd(const void* qkv, void* out, float* lse2, const int* c
   return 0;
 }
 
-}  // namespace vj
-
-extern "C" int vj_attn_fwd(const void* qkv, void* out, float* lse2, const int* cu_seqlens, int nseq, int max_len,
-                           int H, int HD, int T, float scale, void* stream_) {
-  using namespace vj;
-  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream_);
+template <typename T>
+static int attn_fwd_impl(const void* qkv, void* out, float* lse2, const int* cu_seqlens, int nseq, int max_len, int H,
+                         int HD, int T_, float scale, cudaStream_t s) {
   VJ_CHECK_ARG(qkv && out && lse2 && cu_seqlens, "vj_attn_fwd: null pointer");
-  VJ_CHECK_ARG(nseq > 0 && max_len > 0 && H > 0 && T > 0, "vj_attn_fwd: empty problem");
+  VJ_CHECK_ARG(nseq > 0 && max_len > 0 && H > 0 && T_ > 0, "vj_attn_fwd: empty problem");
   VJ_CHECK_ARG((reinterpret_cast<uintptr_t>(qkv) & 15) == 0 && (reinterpret_cast<uintptr_t>(out) & 15) == 0,
                "vj_attn_fwd: pointers must be 16-byte aligned");
   switch (HD) {
-    case 32: return launch_attn_fwd<32>(qkv, out, lse2, cu_seqlens, nseq, max_len, H, T, scale, s);
-    case 64: return launch_attn_fwd<64>(qkv, out, lse2, cu_seqlens, nseq, max_len, H, T, scale, s);
-    case 128: return launch_attn_fwd<128>(qkv, out, lse2, cu_seqlens, nseq, max_len, H, T, scale, s);
+    case 32: return launch_attn_fwd<T, 32>(qkv, out, lse2, cu_seqlens, nseq, max_len, H, T_, scale, s);
+    case 64: return launch_attn_fwd<T, 64>(qkv, out, lse2, cu_seqlens, nseq, max_len, H, T_, scale, s);
+    case 128: return launch_attn_fwd<T, 128>(qkv, out, lse2, cu_seqlens, nseq, max_len, H, T_, scale, s);
     default: set_error("vj_attn_fwd: head dim %d unsupported (32/64/128; pad 24->32 in the weights)", HD); return -1;
   }
+}
+
+}  // namespace vj
+
+extern "C" int vj_attn_fwd(const void* qkv, void* out, float* lse2, const int* cu_seqlens, int nseq, int max_len,
+                           int H, int HD, int T, float scale, void* stream) {
+  return vj::attn_fwd_impl<__nv_bfloat16>(qkv, out, lse2, cu_seqlens, nseq, max_len, H, HD, T, scale,
+                                          reinterpret_cast<cudaStream_t>(stream));
+}
+
+extern "C" int vj_attn_fwd_f16(const void* qkv, void* out, float* lse2, const int* cu_seqlens, int nseq, int max_len,
+                               int H, int HD, int T, float scale, void* stream) {
+  return vj::attn_fwd_impl<__half>(qkv, out, lse2, cu_seqlens, nseq, max_len, H, HD, T, scale,
+                                   reinterpret_cast<cudaStream_t>(stream));
 }

@@ -6,6 +6,7 @@
 
 #include <cuda.h>
 #include <cuda_bf16.h>
+#include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 
@@ -41,7 +42,7 @@ void count_launch(int n);  // bookkeeping for vj_launch_count()
 
 // Encode a 2-D tiled tensor map.  `inner`/`outer` are element counts, `ld_bytes` the byte
 // stride of the outer dimension.  swizzle: 0 none, 1 32B, 2 64B, 3 128B.
-// dtype: 0 bf16, 1 f32.  Returns 0 on success.
+// dtype: 0 bf16, 1 f32, 2 f16.  Returns 0 on success.
 int make_tmap_2d(CUtensorMap* out, const void* ptr, int dtype, uint64_t inner, uint64_t outer,
                  uint64_t ld_bytes, uint32_t box_inner, uint32_t box_outer, int swizzle);
 
@@ -195,6 +196,33 @@ VJ_DEVINL uint32_t mul_bf16x2(uint32_t a, uint32_t b) {
 }
 VJ_DEVINL float bf16_lo(uint32_t v) { return __uint_as_float(v << 16); }
 VJ_DEVINL float bf16_hi(uint32_t v) { return __uint_as_float(v & 0xFFFF0000u); }
+// fp16 pairs (cvt.rn.f16x2.f32): round to nearest even, a value past 65504 becomes +-inf like torch's .half()
+VJ_DEVINL uint32_t pack_f16x2(float lo, float hi) {
+  __half2 v = __floats2half2_rn(lo, hi);
+  return *reinterpret_cast<uint32_t*>(&v);
+}
+VJ_DEVINL float f16_lo(uint32_t v) { return __half2float(__ushort_as_half(static_cast<unsigned short>(v & 0xFFFFu))); }
+VJ_DEVINL float f16_hi(uint32_t v) { return __half2float(__ushort_as_half(static_cast<unsigned short>(v >> 16))); }
+
+// The 16-bit element types of the tensor-core kernels: bf16 (pre-training, and evaluation by default) and fp16 (frozen
+// evaluation under autocast(float16), as the reference's eval loops run).  Elt<T> holds the TMA data type
+// (make_tmap_2d's dtype code) and the packed conversions; wgmma.cuh picks the MMA's type string from T.
+template <typename T>
+struct Elt;
+template <>
+struct Elt<__nv_bfloat16> {
+  static constexpr int kTmap = 0;
+  static VJ_DEVINL uint32_t pack(float lo, float hi) { return pack_bf16x2(lo, hi); }
+  static VJ_DEVINL float lo(uint32_t v) { return bf16_lo(v); }
+  static VJ_DEVINL float hi(uint32_t v) { return bf16_hi(v); }
+};
+template <>
+struct Elt<__half> {
+  static constexpr int kTmap = 2;
+  static VJ_DEVINL uint32_t pack(float lo, float hi) { return pack_f16x2(lo, hi); }
+  static VJ_DEVINL float lo(uint32_t v) { return f16_lo(v); }
+  static VJ_DEVINL float hi(uint32_t v) { return f16_hi(v); }
+};
 
 VJ_DEVINL float gelu_erf(float x) { return 0.5f * x * (1.0f + erff(x * 0.70710678118654752f)); }
 VJ_DEVINL float gelu_erf_grad(float x) {

@@ -1,6 +1,10 @@
 // wgmma GEMM for the V-JEPA hot path (sm_90a).
 //
-//   D[M,N] = epi( alpha * sum_k A[m,k] * B[n,k] )        bf16 operands, fp32 accumulation in registers
+//   D[M,N] = epi( alpha * sum_k A[m,k] * B[n,k] )        bf16 or fp16 operands, fp32 accumulation in registers
+//
+// The element type T of the operands and of every 16-bit D / aux / aux_out is a template parameter: bf16 for
+// pre-training and bf16 evaluation (vj_gemm), fp16 for frozen evaluation under autocast(float16) (vj_gemm_f16, the
+// reference's eval loops).  Only the combinations that evaluation runs are instantiated in fp16.
 //
 // One persistent CTA per SM, warp-specialised, 3 warpgroups, two schedules:
 //
@@ -33,6 +37,8 @@
 #include "common.cuh"
 #include "vjepa_b200.h"
 #include "wgmma.cuh"
+
+#include <type_traits>
 
 namespace vj {
 
@@ -179,7 +185,7 @@ VJ_DEVINL int aux32_row(const GemmParams& p, int row) {
 // Direct-from-register epilogue for fp32 D (plain store, or reduce-add for split-K / stream-K / accumulate) and for the
 // cooperative weight-gradient kernel's bf16 D.  `acc` is one m64nBN fragment whose rows start at r0: the thread holds
 // rows r0 + lane/4 and r0 + lane/4 + 8, column pairs n0 + 8j + 2(lane%4).
-template <int BN, bool OUT_F32, int EPI, bool AUX32>
+template <typename T, int BN, bool OUT_F32, int EPI, bool AUX32>
 VJ_DEVINL void epilogue_direct(const GemmParams& p, const float (&acc)[BN / 2], int r0, int n0, bool add_bias, int lane) {
   constexpr bool kUsesAux = (EPI == VJ_EPI_ADD || EPI == VJ_EPI_DGELU || EPI == VJ_EPI_MUL);
   static_assert(!kUsesAux || AUX32, "bf16 aux goes through the staged epilogue");
@@ -207,8 +213,7 @@ VJ_DEVINL void epilogue_direct(const GemmParams& p, const float (&acc)[BN / 2], 
         if (p.reduce_add) atomicAdd(dst, make_float2(v0, v1));
         else *dst = make_float2(v0, v1);
       } else {
-        *reinterpret_cast<uint32_t*>(reinterpret_cast<__nv_bfloat16*>(p.D) + (long long)row * p.ldd + col) =
-            pack_bf16x2(v0, v1);
+        *reinterpret_cast<uint32_t*>(reinterpret_cast<T*>(p.D) + (long long)row * p.ldd + col) = Elt<T>::pack(v0, v1);
       }
     }
   }
@@ -218,7 +223,7 @@ VJ_DEVINL void epilogue_direct(const GemmParams& p, const float (&acc)[BN / 2], 
 // forward / dgrad kernel: ping-pong (COOP = false) or, for long K, cooperative on a 128 x 256 tile (COOP = true)
 // ---------------------------------------------------------------------------------------------
 // EPI is a compile-time epilogue kind so that e.g. the plain / GELU kernels carry none of the aux code.
-template <int BN, bool COOP, bool B_MN, bool OUT_F32, int EPI, bool AUX32>
+template <typename T, int BN, bool COOP, bool B_MN, bool OUT_F32, int EPI, bool AUX32>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
             const __grid_constant__ CUtensorMap tmD, const __grid_constant__ CUtensorMap tmAux,
@@ -358,7 +363,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
         const int scale_d = (kb > kb0 || kk > 0) ? 1 : 0;
 #pragma unroll
         for (int hh = 0; hh < HALVES; ++hh)
-          wgmma_ss<BN, 0, B_MN ? 1 : 0>(acc[hh], da + ((8192 * hh + kk * 32) >> 4), db + (kob >> 4), scale_d);
+          wgmma_ss<BN, 0, B_MN ? 1 : 0, T>(acc[hh], da + ((8192 * hh + kk * 32) >> 4), db + (kob >> 4), scale_d);
       }
       wgmma_commit();
       wgmma_wait<1>();   // the previous k-block's MMAs have retired: its stage may be refilled
@@ -386,7 +391,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
     if constexpr (!kStaged) {
 #pragma unroll
       for (int hh = 0; hh < HALVES; ++hh)
-        epilogue_direct<BN, OUT_F32, EPI, AUX32>(p, acc[hh], mw + 64 * hh + 16 * warp_in_wg, n0, add_bias, lane);
+        epilogue_direct<T, BN, OUT_F32, EPI, AUX32>(p, acc[hh], mw + 64 * hh + 16 * warp_in_wg, n0, add_bias, lane);
     } else {
       // ---- staged epilogue.  Thread holds rows 16 w + lane/4 (+8, +64, +72) and column pairs 8j + 2(lane%4); under
       // the 128B swizzle the 16-byte chunk j%8 of row r sits at chunk (j%8) ^ (r%8), and r%8 = lane/4 for all four
@@ -421,7 +426,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
             if (kAuxTma) {
               uint32_t x;
               asm volatile("ld.shared.b32 %0, [%1];" : "=r"(x) : "r"(addr) : "memory");
-              apply_aux<EPI>(v0, v1, bf16_lo(x), bf16_hi(x));
+              apply_aux<EPI>(v0, v1, Elt<T>::lo(x), Elt<T>::hi(x));
             } else if (kUsesAux) {
               // (fp32 aux: the patch embedding's positional table, once per encoder forward; the row lookup is
               //  repeated per column pair rather than held in registers across the loop)
@@ -436,12 +441,12 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
               //   VJ_EPI_GELU_GRAD : aux_out = gelu'(pre) (the backward's epilogue is then a plain multiply)
               float d0, d1;
               const float g0 = gelu_and_grad(v0, d0), g1 = gelu_and_grad(v1, d1);
-              o = EPI == VJ_EPI_GELU ? pack_bf16x2(v0, v1) : pack_bf16x2(d0, d1);
+              o = EPI == VJ_EPI_GELU ? Elt<T>::pack(v0, v1) : Elt<T>::pack(d0, d1);
               a0 = g0;
               a1 = g1;
-              if (!two_pass) o = pack_bf16x2(g0, g1);
+              if (!two_pass) o = Elt<T>::pack(g0, g1);
             } else {
-              o = pack_bf16x2(v0, v1);
+              o = Elt<T>::pack(v0, v1);
             }
             asm volatile("st.shared.b32 [%0], %1;" ::"r"(addr), "r"(o) : "memory");
           }
@@ -463,7 +468,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
           for (int hh = 0; hh < HALVES; ++hh)
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
-              const uint32_t o = pack_bf16x2(acc[hh][4 * j + 2 * h], acc[hh][4 * j + 2 * h + 1]);
+              const uint32_t o = Elt<T>::pack(acc[hh][4 * j + 2 * h], acc[hh][4 * j + 2 * h + 1]);
               asm volatile("st.shared.b32 [%0], %1;" ::"r"(cj + (64 * hh + 8 * h) * 128), "r"(o) : "memory");
             }
         }
@@ -486,7 +491,7 @@ gemm_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUt
 // ---------------------------------------------------------------------------------------------
 // cooperative weight-gradient kernel (both operands MN-major, promoted accumulation)
 // ---------------------------------------------------------------------------------------------
-template <int BN, bool OUT_F32>
+template <typename T, int BN, bool OUT_F32>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 gemm_wgrad_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, const GemmParams p) {
   static_assert(BN <= 128, "promoted accumulation needs two accumulator sets in registers");
@@ -571,7 +576,7 @@ gemm_wgrad_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
       wgmma_fence();
 #pragma unroll
       for (int kk = 0; kk < BK / 16; ++kk)
-        wgmma_ss<BN, 1, 1>(part, da0 + ((kk * 2048) >> 4), db0 + ((kk * 2048) >> 4), (!group_first || kk > 0) ? 1 : 0);
+        wgmma_ss<BN, 1, 1, T>(part, da0 + ((kk * 2048) >> 4), db0 + ((kk * 2048) >> 4), (!group_first || kk > 0) ? 1 : 0);
       wgmma_commit();
       if (group_last) {
         wgmma_wait<0>();
@@ -597,7 +602,7 @@ gemm_wgrad_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     if (lane == 0) mbar_arrive(empty0 + 8 * prev);
 
     const bool add_bias = p.bias != nullptr && kb0 == 0;   // the bias joins the piece holding the tile's first k-block
-    epilogue_direct<BN, OUT_F32, VJ_EPI_NONE, false>(p, acc, m0 + cw * 64 + warp_in_wg * 16, n0, add_bias, lane);
+    epilogue_direct<T, BN, OUT_F32, VJ_EPI_NONE, false>(p, acc, m0 + cw * 64 + warp_in_wg * 16, n0, add_bias, lane);
   }
 }
 
@@ -614,13 +619,13 @@ static int grid_size(const GemmParams& p) {
 }
 
 struct GemmMaps {
-  CUtensorMap A, B, D, aux, aux_out;   // D / aux / aux_out: bf16 boxes of the staged epilogue (zero if unused)
+  CUtensorMap A, B, D, aux, aux_out;   // D / aux / aux_out: 16-bit boxes of the staged epilogue (zero if unused)
 };
 
-template <int BN, bool COOP, bool B_MN, bool OUT_F32, int EPI, bool AUX32 = false>
+template <typename T, int BN, bool COOP, bool B_MN, bool OUT_F32, int EPI, bool AUX32 = false>
 static int launch_gemm(const GemmMaps& m, const GemmParams& p, cudaStream_t stream) {
   constexpr int SMEM = PingCfg<BN, !OUT_F32, COOP>::SMEM_BYTES;
-  auto kern = gemm_kernel<BN, COOP, B_MN, OUT_F32, EPI, AUX32>;
+  auto kern = gemm_kernel<T, BN, COOP, B_MN, OUT_F32, EPI, AUX32>;
   static bool configured = false;  // per instantiation
   if (!configured) {
     VJ_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM));
@@ -632,10 +637,10 @@ static int launch_gemm(const GemmMaps& m, const GemmParams& p, cudaStream_t stre
   return 0;
 }
 
-template <int BN, bool OUT_F32>
+template <typename T, int BN, bool OUT_F32>
 static int launch_gemm_wgrad(const GemmMaps& m, const GemmParams& p, cudaStream_t stream) {
   constexpr int SMEM = GemmCfg<BN>::SMEM_BYTES;
-  auto kern = gemm_wgrad_kernel<BN, OUT_F32>;
+  auto kern = gemm_wgrad_kernel<T, BN, OUT_F32>;
   static bool configured = false;  // per instantiation
   if (!configured) {
     VJ_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM));
@@ -647,43 +652,49 @@ static int launch_gemm_wgrad(const GemmMaps& m, const GemmParams& p, cudaStream_
   return 0;
 }
 
-template <int BN, bool COOP>
+template <typename T, int BN, bool COOP>
 static int dispatch_major(int a_mn, int b_mn, int out_f32, int epi, int aux_f32, const GemmMaps& m,
                           const GemmParams& p, cudaStream_t s) {
-  // instantiated combinations = what the V-JEPA step needs (forward Linear: K/K; dgrad: K/MN; wgrad: MN/MN fp32)
+  // instantiated combinations = what the V-JEPA step needs (forward Linear: K/K; dgrad: K/MN; wgrad: MN/MN fp32);
+  // in fp16 only what frozen evaluation runs (the encoder's forward, the probe's forward and backward)
+  constexpr bool kBf16 = std::is_same<T, __nv_bfloat16>::value;
   if (!a_mn && !b_mn) {
-    if (epi == VJ_EPI_NONE) return out_f32 ? launch_gemm<BN, COOP, false, true, VJ_EPI_NONE>(m, p, s)
-                                           : launch_gemm<BN, COOP, false, false, VJ_EPI_NONE>(m, p, s);
+    if (epi == VJ_EPI_NONE) return out_f32 ? launch_gemm<T, BN, COOP, false, true, VJ_EPI_NONE>(m, p, s)
+                                           : launch_gemm<T, BN, COOP, false, false, VJ_EPI_NONE>(m, p, s);
     if (epi == VJ_EPI_ADD) {
-      if (aux_f32) return out_f32 ? launch_gemm<BN, COOP, false, true, VJ_EPI_ADD, true>(m, p, s)
-                                  : launch_gemm<BN, COOP, false, false, VJ_EPI_ADD, true>(m, p, s);
-      if (!out_f32) return launch_gemm<BN, COOP, false, false, VJ_EPI_ADD, false>(m, p, s);
+      if (aux_f32) return out_f32 ? launch_gemm<T, BN, COOP, false, true, VJ_EPI_ADD, true>(m, p, s)
+                                  : launch_gemm<T, BN, COOP, false, false, VJ_EPI_ADD, true>(m, p, s);
+      if (!out_f32) return launch_gemm<T, BN, COOP, false, false, VJ_EPI_ADD, false>(m, p, s);
     }
-    if (epi == VJ_EPI_GELU && !out_f32) return launch_gemm<BN, COOP, false, false, VJ_EPI_GELU>(m, p, s);
-    if (epi == VJ_EPI_GELU_GRAD && !out_f32) return launch_gemm<BN, COOP, false, false, VJ_EPI_GELU_GRAD>(m, p, s);
-    if (epi == VJ_EPI_DGELU && !out_f32 && !aux_f32) return launch_gemm<BN, COOP, false, false, VJ_EPI_DGELU>(m, p, s);
+    if (epi == VJ_EPI_GELU && !out_f32) return launch_gemm<T, BN, COOP, false, false, VJ_EPI_GELU>(m, p, s);
+    if (epi == VJ_EPI_GELU_GRAD && !out_f32) return launch_gemm<T, BN, COOP, false, false, VJ_EPI_GELU_GRAD>(m, p, s);
+    if constexpr (kBf16)
+      if (epi == VJ_EPI_DGELU && !out_f32 && !aux_f32) return launch_gemm<T, BN, COOP, false, false, VJ_EPI_DGELU>(m, p, s);
   } else if (!a_mn && b_mn) {
-    if (epi == VJ_EPI_NONE) return out_f32 ? launch_gemm<BN, COOP, true, true, VJ_EPI_NONE>(m, p, s)
-                                           : launch_gemm<BN, COOP, true, false, VJ_EPI_NONE>(m, p, s);
-    if (epi == VJ_EPI_DGELU && !out_f32 && !aux_f32) return launch_gemm<BN, COOP, true, false, VJ_EPI_DGELU>(m, p, s);
-    if (epi == VJ_EPI_MUL && !out_f32 && !aux_f32) return launch_gemm<BN, COOP, true, false, VJ_EPI_MUL>(m, p, s);
+    if (epi == VJ_EPI_NONE) return out_f32 ? launch_gemm<T, BN, COOP, true, true, VJ_EPI_NONE>(m, p, s)
+                                           : launch_gemm<T, BN, COOP, true, false, VJ_EPI_NONE>(m, p, s);
+    if constexpr (kBf16)
+      if (epi == VJ_EPI_DGELU && !out_f32 && !aux_f32) return launch_gemm<T, BN, COOP, true, false, VJ_EPI_DGELU>(m, p, s);
+    if (epi == VJ_EPI_MUL && !out_f32 && !aux_f32) return launch_gemm<T, BN, COOP, true, false, VJ_EPI_MUL>(m, p, s);
   } else if (a_mn && b_mn) {
     if constexpr (!COOP) {
-      if (epi == VJ_EPI_NONE) return out_f32 ? launch_gemm_wgrad<BN, true>(m, p, s) : launch_gemm_wgrad<BN, false>(m, p, s);
+      if (epi == VJ_EPI_NONE) {
+        if (out_f32) return launch_gemm_wgrad<T, BN, true>(m, p, s);
+        if constexpr (kBf16) return launch_gemm_wgrad<T, BN, false>(m, p, s);
+      }
     }
   }
-  set_error("vj_gemm: combination a_mn=%d b_mn=%d d_f32=%d epi=%d is not instantiated", a_mn, b_mn, out_f32, epi);
+  set_error("vj_gemm%s: combination a_mn=%d b_mn=%d d_f32=%d epi=%d aux_f32=%d is not instantiated", kBf16 ? "" : "_f16",
+            a_mn, b_mn, out_f32, epi, aux_f32);
   return -1;
 }
 
-}  // namespace vj
-
-extern "C" int vj_gemm(const void* A, long long lda, int a_mn, const void* B, long long ldb,
-                       int b_mn, void* D, long long ldd, int d_f32, int M, int N, int K,
-                       const float* bias, float alpha, int epi, const void* aux, long long ldaux,
-                       int aux_f32, const int* aux_rowmap, int aux_period, void* aux_out,
-                       long long ldauxout, int split_k, int accumulate, void* stream_) {
-  using namespace vj;
+template <typename T>
+static int gemm_impl(const void* A, long long lda, int a_mn, const void* B, long long ldb,
+                     int b_mn, void* D, long long ldd, int d_f32, int M, int N, int K,
+                     const float* bias, float alpha, int epi, const void* aux, long long ldaux,
+                     int aux_f32, const int* aux_rowmap, int aux_period, void* aux_out,
+                     long long ldauxout, int split_k, int accumulate, void* stream_) {
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
   VJ_CHECK_ARG(A && B && D, "vj_gemm: null operand");
   VJ_CHECK_ARG(M > 0 && N > 0 && K > 0, "vj_gemm: empty problem M=%d N=%d K=%d", M, N, K);
@@ -757,19 +768,40 @@ extern "C" int vj_gemm(const void* A, long long lda, int a_mn, const void* B, lo
   GemmMaps m;
   memset(&m, 0, sizeof(m));
   int rc;
-  if (!a_mn) rc = make_tmap_2d(&m.A, A, 0, K, M, lda * 2, 64, 128, 3);
-  else       rc = make_tmap_2d(&m.A, A, 0, M, K, lda * 2, 64, 64, 3);
+  constexpr int dt = Elt<T>::kTmap;
+  if (!a_mn) rc = make_tmap_2d(&m.A, A, dt, K, M, lda * 2, 64, 128, 3);
+  else       rc = make_tmap_2d(&m.A, A, dt, M, K, lda * 2, 64, 64, 3);
   if (rc) return rc;
-  if (!b_mn) rc = make_tmap_2d(&m.B, B, 0, K, N, ldb * 2, 64, BN, 3);
-  else       rc = make_tmap_2d(&m.B, B, 0, N, K, ldb * 2, 64, 64, 3);
+  if (!b_mn) rc = make_tmap_2d(&m.B, B, dt, K, N, ldb * 2, 64, BN, 3);
+  else       rc = make_tmap_2d(&m.B, B, dt, N, K, ldb * 2, 64, 64, 3);
   if (rc) return rc;
   if (!(a_mn && b_mn) && !d_f32) {
     const int rows = coop ? 64 : BM;   // staging rows per consumer warpgroup
-    if ((rc = make_tmap_2d(&m.D, D, 0, N, M, ldd * 2, 64, rows, 3))) return rc;
-    if (aux_tma && (rc = make_tmap_2d(&m.aux, aux, 0, N, M, ldaux * 2, 64, rows, 3))) return rc;
-    if (p.aux_out != nullptr && (rc = make_tmap_2d(&m.aux_out, aux_out, 0, N, M, ldauxout * 2, 64, rows, 3))) return rc;
+    if ((rc = make_tmap_2d(&m.D, D, dt, N, M, ldd * 2, 64, rows, 3))) return rc;
+    if (aux_tma && (rc = make_tmap_2d(&m.aux, aux, dt, N, M, ldaux * 2, 64, rows, 3))) return rc;
+    if (p.aux_out != nullptr && (rc = make_tmap_2d(&m.aux_out, aux_out, dt, N, M, ldauxout * 2, 64, rows, 3))) return rc;
   }
-  if (coop) return dispatch_major<256, true>(a_mn, b_mn, d_f32, epi, aux_f32, m, p, stream);
-  return BN == 128 ? dispatch_major<128, false>(a_mn, b_mn, d_f32, epi, aux_f32, m, p, stream)
-                   : dispatch_major<64, false>(a_mn, b_mn, d_f32, epi, aux_f32, m, p, stream);
+  if (coop) return dispatch_major<T, 256, true>(a_mn, b_mn, d_f32, epi, aux_f32, m, p, stream);
+  return BN == 128 ? dispatch_major<T, 128, false>(a_mn, b_mn, d_f32, epi, aux_f32, m, p, stream)
+                   : dispatch_major<T, 64, false>(a_mn, b_mn, d_f32, epi, aux_f32, m, p, stream);
+}
+
+}  // namespace vj
+
+extern "C" int vj_gemm(const void* A, long long lda, int a_mn, const void* B, long long ldb,
+                       int b_mn, void* D, long long ldd, int d_f32, int M, int N, int K,
+                       const float* bias, float alpha, int epi, const void* aux, long long ldaux,
+                       int aux_f32, const int* aux_rowmap, int aux_period, void* aux_out,
+                       long long ldauxout, int split_k, int accumulate, void* stream) {
+  return vj::gemm_impl<__nv_bfloat16>(A, lda, a_mn, B, ldb, b_mn, D, ldd, d_f32, M, N, K, bias, alpha, epi, aux, ldaux,
+                                      aux_f32, aux_rowmap, aux_period, aux_out, ldauxout, split_k, accumulate, stream);
+}
+
+extern "C" int vj_gemm_f16(const void* A, long long lda, int a_mn, const void* B, long long ldb,
+                           int b_mn, void* D, long long ldd, int d_f32, int M, int N, int K,
+                           const float* bias, float alpha, int epi, const void* aux, long long ldaux,
+                           int aux_f32, const int* aux_rowmap, int aux_period, void* aux_out,
+                           long long ldauxout, int split_k, int accumulate, void* stream) {
+  return vj::gemm_impl<__half>(A, lda, a_mn, B, ldb, b_mn, D, ldd, d_f32, M, N, K, bias, alpha, epi, aux, ldaux,
+                               aux_f32, aux_rowmap, aux_period, aux_out, ldauxout, split_k, accumulate, stream);
 }

@@ -6,35 +6,44 @@
 #include "common.cuh"
 #include "vjepa_b200.h"
 
+#include <type_traits>
+
 namespace vj {
 
-template <bool F32>
+// Storage type codes of the row kernels, the values of the ABI's x_f32 / y_f32 flags: 0 bf16, 1 fp32, 2 fp16
+// (frozen evaluation under autocast(float16)).  `true` / `false` template arguments read as fp32 / bf16.
+template <int DT>
+using Half16 = typename std::conditional<DT == 2, __half, __nv_bfloat16>::type;
+
+template <int DT>
 VJ_DEVINL void ld8(const void* base, long long off, float (&v)[8]) {
-  if (F32) {
+  if (DT == 1) {
     const float4* p = reinterpret_cast<const float4*>(reinterpret_cast<const float*>(base) + off);
     const float4 a = p[0], b = p[1];
     v[0] = a.x; v[1] = a.y; v[2] = a.z; v[3] = a.w; v[4] = b.x; v[5] = b.y; v[6] = b.z; v[7] = b.w;
   } else {
-    const uint4 u = *reinterpret_cast<const uint4*>(reinterpret_cast<const __nv_bfloat16*>(base) + off);
-    v[0] = bf16_lo(u.x); v[1] = bf16_hi(u.x); v[2] = bf16_lo(u.y); v[3] = bf16_hi(u.y);
-    v[4] = bf16_lo(u.z); v[5] = bf16_hi(u.z); v[6] = bf16_lo(u.w); v[7] = bf16_hi(u.w);
+    using E = Elt<Half16<DT>>;
+    const uint4 u = *reinterpret_cast<const uint4*>(reinterpret_cast<const uint16_t*>(base) + off);
+    v[0] = E::lo(u.x); v[1] = E::hi(u.x); v[2] = E::lo(u.y); v[3] = E::hi(u.y);
+    v[4] = E::lo(u.z); v[5] = E::hi(u.z); v[6] = E::lo(u.w); v[7] = E::hi(u.w);
   }
 }
-template <bool F32>
+template <int DT>
 VJ_DEVINL void st8(void* base, long long off, const float (&v)[8]) {
-  if (F32) {
+  if (DT == 1) {
     float4* p = reinterpret_cast<float4*>(reinterpret_cast<float*>(base) + off);
     p[0] = make_float4(v[0], v[1], v[2], v[3]);
     p[1] = make_float4(v[4], v[5], v[6], v[7]);
   } else {
+    using E = Elt<Half16<DT>>;
     uint4 u;
-    u.x = pack_bf16x2(v[0], v[1]); u.y = pack_bf16x2(v[2], v[3]);
-    u.z = pack_bf16x2(v[4], v[5]); u.w = pack_bf16x2(v[6], v[7]);
-    *reinterpret_cast<uint4*>(reinterpret_cast<__nv_bfloat16*>(base) + off) = u;
+    u.x = E::pack(v[0], v[1]); u.y = E::pack(v[2], v[3]);
+    u.z = E::pack(v[4], v[5]); u.w = E::pack(v[6], v[7]);
+    *reinterpret_cast<uint4*>(reinterpret_cast<uint16_t*>(base) + off) = u;
   }
 }
 
-template <int NV, bool IN_F32, bool OUT_F32>
+template <int NV, int IN_F32, int OUT_F32>
 __global__ void __launch_bounds__(256, NV <= 2 ? 4 : (NV <= 4 ? 3 : 1))
 ln_fwd_kernel(const void* __restrict__ x, void* __restrict__ y, const float* __restrict__ gamma,
               const float* __restrict__ beta, float* __restrict__ mean_out, float* __restrict__ rstd_out, int T, int D,
@@ -456,7 +465,11 @@ template <int NV>
 static void launch_ln_fwd(const void* x, int x_f32, void* y, int y_f32, const float* gamma, const float* beta, float* mean,
                           float* rstd, int T, int D, float eps, cudaStream_t s) {
   const int grid = ln_grid(T);
-  if (x_f32 && y_f32) ln_fwd_kernel<NV, true, true><<<grid, 256, 0, s>>>(x, y, gamma, beta, mean, rstd, T, D, eps);
+  if (x_f32 == 2 || y_f32 == 2) {   // fp16 (evaluation under autocast(float16)): fp16 -> fp16 / fp32, fp32 -> fp16
+    if (x_f32 == 2 && y_f32 == 2) ln_fwd_kernel<NV, 2, 2><<<grid, 256, 0, s>>>(x, y, gamma, beta, mean, rstd, T, D, eps);
+    else if (x_f32 == 2) ln_fwd_kernel<NV, 2, 1><<<grid, 256, 0, s>>>(x, y, gamma, beta, mean, rstd, T, D, eps);
+    else ln_fwd_kernel<NV, 1, 2><<<grid, 256, 0, s>>>(x, y, gamma, beta, mean, rstd, T, D, eps);
+  } else if (x_f32 && y_f32) ln_fwd_kernel<NV, true, true><<<grid, 256, 0, s>>>(x, y, gamma, beta, mean, rstd, T, D, eps);
   else if (x_f32) ln_fwd_kernel<NV, true, false><<<grid, 256, 0, s>>>(x, y, gamma, beta, mean, rstd, T, D, eps);
   else if (y_f32) ln_fwd_kernel<NV, false, true><<<grid, 256, 0, s>>>(x, y, gamma, beta, mean, rstd, T, D, eps);
   else {
@@ -524,6 +537,8 @@ extern "C" int vj_layernorm_fwd(const void* x, int x_f32, void* y, int y_f32, co
   if (T <= 0) return 0;
   VJ_CHECK_ARG(x && y && gamma && beta, "vj_layernorm_fwd: null pointer");
   VJ_CHECK_ARG(D % 8 == 0 && D <= 2048, "vj_layernorm_fwd: D=%d unsupported (multiple of 8, <= 2048)", D);
+  VJ_CHECK_ARG(x_f32 >= 0 && x_f32 <= 2 && y_f32 >= 0 && y_f32 <= 2 && !((x_f32 == 2) != (y_f32 == 2) && x_f32 + y_f32 != 3),
+               "vj_layernorm_fwd: x_f32=%d y_f32=%d (0 bf16, 1 fp32, 2 fp16; fp16 pairs with fp16 or fp32)", x_f32, y_f32);
 #define VJ_CALL(NV) launch_ln_fwd<NV>(x, x_f32, y, y_f32, gamma, beta, mean, rstd, T, D, eps, s)
   VJ_LN_DISPATCH(D, VJ_CALL);
 #undef VJ_CALL

@@ -15,13 +15,14 @@ static int flat_grid(long long n_vec, int threads) {
   return int(g);
 }
 
-__global__ void __launch_bounds__(256) cast_f32_bf16_kernel(const float4* __restrict__ src, uint2* __restrict__ dst,
+template <typename TO>
+__global__ void __launch_bounds__(256) cast_f32_kernel(const float4* __restrict__ src, uint2* __restrict__ dst,
                                                             long long n4) {
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n4; i += (long long)gridDim.x * blockDim.x) {
     const float4 f = src[i];
     uint2 o;
-    o.x = pack_bf16x2(f.x, f.y);
-    o.y = pack_bf16x2(f.z, f.w);
+    o.x = Elt<TO>::pack(f.x, f.y);
+    o.y = Elt<TO>::pack(f.z, f.w);
     dst[i] = o;
   }
 }
@@ -122,17 +123,25 @@ __global__ void __launch_bounds__(256) sumsq_kernel(const float4* __restrict__ x
 
 using namespace vj;
 
-extern "C" int vj_cast_f32_bf16(const float* src, void* dst, long long n, void* stream_) {
-  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream_);
+template <typename TO>
+static int cast_f32(const float* src, void* dst, long long n, cudaStream_t s) {
   VJ_CHECK_ARG(src && dst, "vj_cast_f32_bf16: null pointer");
   VJ_CHECK_ARG(n % 4 == 0 && (reinterpret_cast<uintptr_t>(src) & 15) == 0 && (reinterpret_cast<uintptr_t>(dst) & 7) == 0,
                "vj_cast_f32_bf16: n %% 4 and 16-byte alignment required");
   if (n <= 0) return 0;
-  cast_f32_bf16_kernel<<<flat_grid(n / 4, 256), 256, 0, s>>>(reinterpret_cast<const float4*>(src),
-                                                              reinterpret_cast<uint2*>(dst), n / 4);
+  cast_f32_kernel<TO><<<flat_grid(n / 4, 256), 256, 0, s>>>(reinterpret_cast<const float4*>(src),
+                                                                  reinterpret_cast<uint2*>(dst), n / 4);
   VJ_CUDA(cudaGetLastError());
   vj::count_launch(1);
   return 0;
+}
+
+extern "C" int vj_cast_f32_bf16(const float* src, void* dst, long long n, void* stream) {
+  return cast_f32<__nv_bfloat16>(src, dst, n, reinterpret_cast<cudaStream_t>(stream));
+}
+
+extern "C" int vj_cast_f32_f16(const float* src, void* dst, long long n, void* stream) {
+  return cast_f32<__half>(src, dst, n, reinterpret_cast<cudaStream_t>(stream));
 }
 
 extern "C" int vj_head_pad(const void* src, int src_f32, void* dst, int dst_f32, long long outer, int G, int hd, int hdp,
@@ -140,13 +149,16 @@ extern "C" int vj_head_pad(const void* src, int src_f32, void* dst, int dst_f32,
   cudaStream_t s = reinterpret_cast<cudaStream_t>(stream_);
   VJ_CHECK_ARG(src && dst, "vj_head_pad: null pointer");
   VJ_CHECK_ARG(hd > 0 && hdp >= hd && G > 0 && outer > 0 && inner > 0, "vj_head_pad: bad geometry");
+  VJ_CHECK_ARG(dst_f32 != 2 || (src_f32 == 1 && !unpad_add), "vj_head_pad: an fp16 destination takes an fp32 source");
   if (unpad_add) {
     VJ_CHECK_ARG(src_f32 && dst_f32, "vj_head_pad: unpad-add is fp32 only");
     head_unpad_add_kernel<<<flat_grid(outer * G * hd * inner, 256), 256, 0, s>>>(
         reinterpret_cast<const float*>(src), reinterpret_cast<float*>(dst), outer, G, hd, hdp, inner);
   } else {
     const int g = flat_grid(outer * G * hdp * inner, 256);
-    if (src_f32 && dst_f32)
+    if (dst_f32 == 2)
+      head_pad_kernel<float, __half><<<g, 256, 0, s>>>(reinterpret_cast<const float*>(src), reinterpret_cast<__half*>(dst), outer, G, hd, hdp, inner);
+    else if (src_f32 && dst_f32)
       head_pad_kernel<float, float><<<g, 256, 0, s>>>(reinterpret_cast<const float*>(src), reinterpret_cast<float*>(dst), outer, G, hd, hdp, inner);
     else if (src_f32)
       head_pad_kernel<float, __nv_bfloat16><<<g, 256, 0, s>>>(reinterpret_cast<const float*>(src), reinterpret_cast<__nv_bfloat16*>(dst), outer, G, hd, hdp, inner);

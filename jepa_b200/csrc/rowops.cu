@@ -79,7 +79,8 @@ __global__ void __launch_bounds__(256) colsum_kernel(const void* __restrict__ in
 // (c, dt, dh, dw) = Conv3d weight flattening; row = (b, token) with token = (t', h', w') row-major
 // or the gathered token idx[b, k].  One warp per (row, c, dt) slab of ps*ps contiguous outputs.
 // =============================================================================================
-__global__ void __launch_bounds__(256) im2col_kernel(const float* __restrict__ clips, __nv_bfloat16* __restrict__ out,
+template <typename TO>
+__global__ void __launch_bounds__(256) im2col_kernel(const float* __restrict__ clips, TO* __restrict__ out,
                                                      const long long* __restrict__ idx, int B, int C, int T, int H,
                                                      int W, int tub, int ps, int tokens_per_clip_out, int n_tokens) {
   const int gh = H / ps, gw = W / ps;
@@ -99,14 +100,14 @@ __global__ void __launch_bounds__(256) im2col_kernel(const float* __restrict__ c
     const int c = slab / tub, dt = slab % tub;
     const int tw = int(tok % gw), th = int((tok / gw) % gh), tt = int(tok / ((long long)gw * gh));
     const float* src = clips + ((((long long)b * C + c) * T + (tt * tub + dt)) * H + (long long)th * ps) * W + tw * ps;
-    __nv_bfloat16* dst = out + row * P + (long long)slab * ps * ps;
+    TO* dst = out + row * P + (long long)slab * ps * ps;
     // ps*ps elements: dh rows of ps contiguous floats
     for (int e = lane * 4; e < ps * ps; e += 128) {
       const int dh = e / ps, dw = e % ps;
       const float4 f = *reinterpret_cast<const float4*>(src + (long long)dh * W + dw);
       uint2 o;
-      o.x = pack_bf16x2(f.x, f.y);
-      o.y = pack_bf16x2(f.z, f.w);
+      o.x = Elt<TO>::pack(f.x, f.y);
+      o.y = Elt<TO>::pack(f.z, f.w);
       *reinterpret_cast<uint2*>(dst + e) = o;
     }
   }
@@ -490,9 +491,9 @@ extern "C" int vj_colsum(const void* in, int in_f32, float* out, long long T, in
   return 0;
 }
 
-extern "C" int vj_im2col_tubelets(const float* clips, void* patches, const long long* idx, int B, int C, int T, int H,
-                                  int W, int tubelet, int patch, int K, void* stream_) {
-  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream_);
+template <typename TO>
+static int im2col_tubelets(const float* clips, void* patches, const long long* idx, int B, int C, int T, int H, int W,
+                           int tubelet, int patch, int K, cudaStream_t s) {
   VJ_CHECK_ARG(clips && patches, "vj_im2col_tubelets: null pointer");
   VJ_CHECK_ARG(T % tubelet == 0 && H % patch == 0 && W % patch == 0 && patch % 4 == 0 && W % 4 == 0,
                "vj_im2col_tubelets: bad geometry");
@@ -500,11 +501,23 @@ extern "C" int vj_im2col_tubelets(const float* clips, void* patches, const long 
   const int kout = idx ? K : n_tokens;
   if (B <= 0 || kout <= 0) return 0;
   const long long warps = (long long)B * kout * C * tubelet;
-  im2col_kernel<<<grid_for(warps, 8), 256, 0, s>>>(clips, reinterpret_cast<__nv_bfloat16*>(patches), idx, B, C, T, H,
-                                                   W, tubelet, patch, kout, n_tokens);
+  im2col_kernel<TO><<<grid_for(warps, 8), 256, 0, s>>>(clips, reinterpret_cast<TO*>(patches), idx, B, C, T, H, W,
+                                                       tubelet, patch, kout, n_tokens);
   VJ_CUDA(cudaGetLastError());
   vj::count_launch(1);
   return 0;
+}
+
+extern "C" int vj_im2col_tubelets(const float* clips, void* patches, const long long* idx, int B, int C, int T, int H,
+                                  int W, int tubelet, int patch, int K, void* stream) {
+  return im2col_tubelets<__nv_bfloat16>(clips, patches, idx, B, C, T, H, W, tubelet, patch, K,
+                                        reinterpret_cast<cudaStream_t>(stream));
+}
+
+extern "C" int vj_im2col_tubelets_f16(const float* clips, void* patches, const long long* idx, int B, int C, int T,
+                                      int H, int W, int tubelet, int patch, int K, void* stream) {
+  return im2col_tubelets<__half>(clips, patches, idx, B, C, T, H, W, tubelet, patch, K,
+                                 reinterpret_cast<cudaStream_t>(stream));
 }
 
 extern "C" int vj_gather_rows(const void* x, void* out, const long long* idx, int B, int N, int K, int row_bytes,

@@ -17,7 +17,7 @@ import torch
 from . import kernels as K
 from .params import padded_head_dim
 
-BF16, F32 = torch.bfloat16, torch.float32
+BF16, F16, F32 = torch.bfloat16, torch.float16, torch.float32
 LN_EPS = 1e-6  # norm_layer=partial(nn.LayerNorm, eps=1e-6): vision_transformer.py:252, predictor.py:244
 
 
@@ -86,8 +86,8 @@ class StackSpec:
         self.block_prefix = block_prefix       # e.g. "blocks" / "predictor_blocks"
 
 
-def gather_block_weights(store, spec, scratch):
-    """Collect bf16 weights for every block; builds head-padded copies when hd is not a tile size."""
+def gather_block_weights(store, spec, scratch, dtype=BF16):
+    """Collect the `dtype` (bf16 or fp16) weights of every block; builds head-padded copies when hd is not a tile size."""
     out = []
     dev = store.flat.device
     for i in range(spec.depth):
@@ -96,19 +96,19 @@ def gather_block_weights(store, spec, scratch):
         w.prefix = pre
         w.n1w, w.n1b = store.f32(pre + "norm1.weight"), store.f32(pre + "norm1.bias")
         w.n2w, w.n2b = store.f32(pre + "norm2.weight"), store.f32(pre + "norm2.bias")
-        w.fc1_w, w.fc1_b = store.bf16(pre + "mlp.fc1.weight"), store.f32(pre + "mlp.fc1.bias")
-        w.fc2_w, w.fc2_b = store.bf16(pre + "mlp.fc2.weight"), store.f32(pre + "mlp.fc2.bias")
+        w.fc1_w, w.fc1_b = store.w16(pre + "mlp.fc1.weight", dtype), store.f32(pre + "mlp.fc1.bias")
+        w.fc2_w, w.fc2_b = store.w16(pre + "mlp.fc2.weight", dtype), store.f32(pre + "mlp.fc2.bias")
         w.proj_b = store.f32(pre + "attn.proj.bias")
         if not spec.padded:
-            w.qkv_w, w.qkv_b = store.bf16(pre + "attn.qkv.weight"), store.f32(pre + "attn.qkv.bias")
-            w.proj_w = store.bf16(pre + "attn.proj.weight")
+            w.qkv_w, w.qkv_b = store.w16(pre + "attn.qkv.weight", dtype), store.f32(pre + "attn.qkv.bias")
+            w.proj_w = store.w16(pre + "attn.proj.weight", dtype)
         else:
             H, hd, hdp, D = spec.heads, spec.hd, spec.hdp, spec.dim
-            key = ("pad", i)
+            key = ("pad", i) if dtype == BF16 else ("pad", i, dtype)
             bufs = scratch.get(key)
             if bufs is None:
-                bufs = (_empty((3 * H * hdp, D), BF16, dev), _empty((3 * H * hdp,), F32, dev),
-                        _empty((D, H * hdp), BF16, dev))
+                bufs = (_empty((3 * H * hdp, D), dtype, dev), _empty((3 * H * hdp,), F32, dev),
+                        _empty((D, H * hdp), dtype, dev))
                 scratch[key] = bufs
             K.head_pad(store.f32(pre + "attn.qkv.weight"), bufs[0], 1, 3 * H, hd, hdp, D)
             K.head_pad(store.f32(pre + "attn.qkv.bias"), bufs[1], 1, 3 * H, hd, hdp, 1)
@@ -123,24 +123,25 @@ class BlockSaved:
 
 
 def blocks_forward(spec, weights, x, seq, save, tap=None):
-    """Run the Block stack over token matrix x [T, dim] (bf16).  Returns (x_out, saved list or None).
+    """Run the Block stack over token matrix x [T, dim] (bf16, or fp16 with fp16 weights: the residual stream of the
+    reference's blocks under autocast(float16)).  Returns (x_out, saved list or None).
 
     Block.forward (modules.py:114-120): x = x + proj(attn(LN1(x))); x = x + fc2(gelu(fc1(LN2(x)))).
     tap(i, x): called with the residual stream after block i (multi-layer feature taps, vision_transformer.py:186-187).
     """
     cu, nseq, max_len, T = seq
-    dev = x.device
+    dev, dt = x.device, x.dtype
     D, Hd, W = spec.dim, spec.hidden, spec.inner
     saved = [] if save else None
     # scratch reused across layers when nothing has to be kept for a backward
     ln = qkv = attn = lse = g = None
     for w in weights:
         if save or ln is None:
-            ln = _empty((T, D), BF16, dev)
-            qkv = _empty((T, 3 * W), BF16, dev)
-            attn = _empty((T, W), BF16, dev)
+            ln = _empty((T, D), dt, dev)
+            qkv = _empty((T, 3 * W), dt, dev)
+            attn = _empty((T, W), dt, dev)
             lse = _empty((spec.heads, T), F32, dev)
-            g = _empty((T, Hd), BF16, dev)
+            g = _empty((T, Hd), dt, dev)
         s = None
         if save:
             s = BlockSaved()
@@ -150,14 +151,14 @@ def blocks_forward(spec, weights, x, seq, save, tap=None):
         K.layernorm_fwd(x, ln, w.n1w, w.n1b, LN_EPS, s.mean1 if save else None, s.rstd1 if save else None)
         K.gemm(ln, w.qkv_w, qkv, bias=w.qkv_b)
         K.attn_fwd(qkv, attn, lse, cu, nseq, max_len, spec.heads, spec.hdp, spec.scale)
-        x_mid = _empty((T, D), BF16, dev)
+        x_mid = _empty((T, D), dt, dev)
         K.gemm(attn, w.proj_w, x_mid, bias=w.proj_b, epi=K.EPI_ADD, aux=x)
-        ln2 = _empty((T, D), BF16, dev) if save else ln
+        ln2 = _empty((T, D), dt, dev) if save else ln
         K.layernorm_fwd(x_mid, ln2, w.n2w, w.n2b, LN_EPS, s.mean2 if save else None, s.rstd2 if save else None)
-        h = _empty((T, Hd), BF16, dev) if save else None
+        h = _empty((T, Hd), dt, dev) if save else None
         # training: keep gelu'(pre-activation) (bf16) instead of the pre-activation itself, computed in the same epilogue
         K.gemm(ln2, w.fc1_w, g, bias=w.fc1_b, epi=K.EPI_GELU_GRAD if save else K.EPI_GELU, aux_out=h)
-        x_out = _empty((T, D), BF16, dev)
+        x_out = _empty((T, D), dt, dev)
         K.gemm(g, w.fc2_w, x_out, bias=w.fc2_b, epi=K.EPI_ADD, aux=x_mid)
         if save:
             s.ln1, s.qkv, s.attn, s.lse, s.x_mid, s.ln2, s.h, s.g = ln, qkv, attn, lse, x_mid, ln2, h, g
@@ -248,6 +249,12 @@ class EncoderSaved:
     pass
 
 
+def _norm_dtype(x):
+    """dtype of a final / out_layers norm of the residual stream x: bf16 in a bf16 forward; fp32 in an fp16 one, as
+    nn.LayerNorm returns under autocast(float16) (layer_norm is on autocast's fp32 list)."""
+    return F32 if x.dtype == F16 else x.dtype
+
+
 class _LayerTaps:
     """Collects norm(x) after the requested blocks (out_layers, vision_transformer.py:183-190)."""
 
@@ -256,7 +263,7 @@ class _LayerTaps:
 
     def __call__(self, i, x):
         if i in self.layers:
-            y = torch.empty_like(x)
+            y = torch.empty_like(x, dtype=_norm_dtype(x))
             K.layernorm_fwd(x, y, self.store.f32("norm.weight"), self.store.f32("norm.bias"), LN_EPS, None, None)
             self.outs.append(y)
 
@@ -290,16 +297,25 @@ def encoder_forward(mod, clips, masks, save, final_norm=True, out_layers=None, g
     clips fp32 [B,3,T,H,W] holding whole patches of the token grid `grid` = (T', H', W') (default: the grid the encoder
     was built for); masks: None or list of int64 [B,K_i] indexing that grid.  Returns (out, saved) where out is
     bf16 [sum_i B*K_i, D] (normalised if final_norm else the raw residual stream).
+
+    Under autocast(float16) (the reference's eval loops) the GEMMs, attention and residual stream run in fp16 and the
+    normalised outputs are fp32, the dtypes the reference's modules produce there.  That is a frozen-encoder forward
+    only: `save` (training the encoder) raises.
     """
+    dt = K.compute_dtype()
+    if save and dt == F16:
+        raise NotImplementedError(
+            "training the encoder under autocast(float16) is not supported: the fp16 path is the frozen encoder of "
+            "evaluation, run under torch.no_grad() (train in bf16, or freeze the encoder)")
     store = mod._store.adopt(mod)
-    store.refresh_shadow()
+    store.refresh_shadow(dt)
     spec = mod._spec
     dev = clips.device
     B = clips.shape[0]
     grid = mod.grid if grid is None else tuple(grid)
     N, D = grid[0] * grid[1] * grid[2], mod.embed_dim
     P = mod.patch_embed.proj.weight[0].numel()
-    weights = gather_block_weights(store, spec, mod._scratch)
+    weights = gather_block_weights(store, spec, mod._scratch, dt)
     clips = clips.contiguous()
     if clips.dtype != F32:
         clips = clips.float()
@@ -307,7 +323,7 @@ def encoder_forward(mod, clips, masks, save, final_norm=True, out_layers=None, g
         segments = [(B, N)]
         seq = cu_seqlens_for(segments, dev)
         T = seq[3]
-        patches = _empty((T, P), BF16, dev)
+        patches = _empty((T, P), dt, dev)
         K.im2col_tubelets(clips, patches, None, mod.tubelet_size, mod.patch_size)
         rowmap, period = None, N
     else:
@@ -315,7 +331,7 @@ def encoder_forward(mod, clips, masks, save, final_norm=True, out_layers=None, g
         segments = [(B, int(m.shape[1])) for m in masks]
         seq = cu_seqlens_for(segments, dev)
         T = seq[3]
-        patches = _empty((T, P), BF16, dev)
+        patches = _empty((T, P), dt, dev)
         off = 0
         for m in masks:
             n = B * m.shape[1]
@@ -323,8 +339,8 @@ def encoder_forward(mod, clips, masks, save, final_norm=True, out_layers=None, g
             off += n
         rowmap = torch.cat([m.reshape(-1) for m in masks]).to(torch.int32)
         period = 0
-    x = _empty((T, D), BF16, dev)
-    w_pe = store.bf16("patch_embed.proj.weight").view(D, P)
+    x = _empty((T, D), dt, dev)
+    w_pe = store.w16("patch_embed.proj.weight", dt).view(D, P)
     pos = encoder_pos(mod, store, grid, dev)
     K.gemm(patches, w_pe, x, bias=store.f32("patch_embed.proj.bias"), epi=K.EPI_ADD, aux=pos, aux_rowmap=rowmap,
            aux_period=period)
@@ -341,7 +357,7 @@ def encoder_forward(mod, clips, masks, save, final_norm=True, out_layers=None, g
         sv = EncoderSaved()
         sv.patches, sv.seq, sv.blocks, sv.weights, sv.x_final, sv.store = patches, seq, bsaved, weights, x, store
     if final_norm:
-        out = _empty((T, D), BF16, dev)
+        out = _empty((T, D), _norm_dtype(x), dev)
         mean = _empty((T,), F32, dev) if save else None
         rstd = _empty((T,), F32, dev) if save else None
         K.layernorm_fwd(x, out, store.f32("norm.weight"), store.f32("norm.bias"), LN_EPS, mean, rstd)
@@ -383,6 +399,10 @@ def predictor_forward(mod, z_cat, masks_ctxt, masks_tgt, mask_indices, save):
     z_cat bf16 [sum_i B*Ke_i, D_enc]: context tokens of every mask, concatenated in mask order.
     Returns (pred bf16 [sum_i B*Kp_i, D_enc], saved).
     """
+    if K.compute_dtype() == F16:
+        raise NotImplementedError(
+            "the predictor does not run under autocast(float16): fp16 covers the frozen encoder of evaluation only "
+            "(pre-training computes in bf16)")
     store = mod._store.adopt(mod)
     store.refresh_shadow()
     spec = mod._spec

@@ -10,7 +10,16 @@ import torch
 from . import _lib
 
 EPI_NONE, EPI_GELU, EPI_ADD, EPI_DGELU, EPI_MUL, EPI_GELU_GRAD = 0, 1, 2, 3, 4, 5
-BF16, F32 = torch.bfloat16, torch.float32
+BF16, F16, F32 = torch.bfloat16, torch.float16, torch.float32
+
+
+def compute_dtype():
+    """Element type of the tensor-core operands for the caller's autocast state: fp16 inside
+    torch.autocast('cuda', dtype=torch.float16) (or the deprecated torch.cuda.amp.autocast(dtype=torch.float16)), as the
+    reference's eval loops run their frozen encoder; bf16 everywhere else (no autocast, or bf16 autocast)."""
+    if torch.is_autocast_enabled("cuda") and torch.get_autocast_dtype("cuda") == F16:
+        return F16
+    return BF16
 
 
 def _s():
@@ -39,10 +48,29 @@ def _isf32(t):
     raise _lib.VJError(f"unsupported dtype {t.dtype}")
 
 
+def _dtcode(t):
+    """The dtype flag of the entry points that also take fp16 (x_f32 / y_f32 / dst_f32): 0 bf16, 1 fp32, 2 fp16."""
+    return 2 if t.dtype == F16 else _isf32(t)
+
+
+def _f16(name, t):
+    """Entry point `name`, or its fp16 twin `name_f16` when the 16-bit operand t is fp16."""
+    if t.dtype == F16:
+        return name + "_f16"
+    if t.dtype != BF16:
+        raise _lib.VJError(f"{name}: 16-bit operand must be bf16 or fp16, got {t.dtype}")
+    return name
+
+
 def gemm(a, b, out, *, a_mn=False, b_mn=False, bias=None, alpha=1.0, epi=EPI_NONE, aux=None, aux_rowmap=None,
          aux_period=0, aux_out=None, split_k=1, accumulate=False):
-    """out[M,N] = epi(alpha * A @ B^T).  a: [M,K] (or [K,M] if a_mn); b: [N,K] (or [K,N] if b_mn)."""
-    _chk(a, BF16, "a"); _chk(b, BF16, "b"); _chk(out, None, "out")
+    """out[M,N] = epi(alpha * A @ B^T).  a: [M,K] (or [K,M] if a_mn); b: [N,K] (or [K,N] if b_mn).
+    a and b are both bf16 or both fp16; a 16-bit out / aux / aux_out has their dtype."""
+    name = _f16("vj_gemm", a)
+    dt = a.dtype
+    _chk(a, dt, "a"); _chk(b, dt, "b"); _chk(out, None, "out")
+    if out.dtype not in (dt, F32):
+        raise _lib.VJError(f"gemm: out must be {dt} or fp32, got {out.dtype}")
     if a_mn:
         K, M = a.shape
     else:
@@ -57,22 +85,26 @@ def gemm(a, b, out, *, a_mn=False, b_mn=False, bias=None, alpha=1.0, epi=EPI_NON
         _chk(bias, F32, "bias")
     if aux is not None:
         _chk(aux, None, "aux")
+        if aux.dtype not in (dt, F32):
+            raise _lib.VJError(f"gemm: aux must be {dt} or fp32, got {aux.dtype}")
     if aux_rowmap is not None:
         _chk(aux_rowmap, torch.int32, "aux_rowmap")
     if aux_out is not None:
-        _chk(aux_out, BF16, "aux_out")
-    _lib.call("vj_gemm", _p(a), a.stride(0), int(a_mn), _p(b), b.stride(0), int(b_mn), _p(out), out.stride(0),
-              _isf32(out), M, N, K, _p(bias), float(alpha), int(epi), _p(aux),
-              aux.stride(0) if aux is not None else 0, _isf32(aux) if aux is not None else 0, _p(aux_rowmap),
+        _chk(aux_out, dt, "aux_out")
+    _lib.call(name, _p(a), a.stride(0), int(a_mn), _p(b), b.stride(0), int(b_mn), _p(out), out.stride(0),
+              int(out.dtype == F32), M, N, K, _p(bias), float(alpha), int(epi), _p(aux),
+              aux.stride(0) if aux is not None else 0, int(aux is not None and aux.dtype == F32), _p(aux_rowmap),
               int(aux_period), _p(aux_out), aux_out.stride(0) if aux_out is not None else 0, int(split_k),
               int(accumulate), _s())
     return out
 
 
 def attn_fwd(qkv, out, lse2, cu_seqlens, nseq, max_len, H, HD, scale):
-    _chk(qkv, BF16, "qkv"); _chk(out, BF16, "out"); _chk(lse2, F32, "lse2"); _chk(cu_seqlens, torch.int32, "cu_seqlens")
+    """qkv and out bf16, or both fp16."""
+    name = _f16("vj_attn_fwd", qkv)
+    _chk(qkv, None, "qkv"); _chk(out, qkv.dtype, "out"); _chk(lse2, F32, "lse2"); _chk(cu_seqlens, torch.int32, "cu_seqlens")
     T = qkv.shape[0]
-    _lib.call("vj_attn_fwd", _p(qkv), _p(out), _p(lse2), _p(cu_seqlens), nseq, max_len, H, HD, T, float(scale), _s())
+    _lib.call(name, _p(qkv), _p(out), _p(lse2), _p(cu_seqlens), nseq, max_len, H, HD, T, float(scale), _s())
     return out
 
 
@@ -91,7 +123,7 @@ def attn_bwd(qkv, out, dout, lse2, delta_ws, dqkv, cu_seqlens, nseq, max_len, H,
 def layernorm_fwd(x, y, gamma, beta, eps, mean=None, rstd=None):
     _chk(x, None, "x"); _chk(y, None, "y"); _chk(gamma, F32, "gamma"); _chk(beta, F32, "beta")
     T, D = x.shape
-    _lib.call("vj_layernorm_fwd", _p(x), _isf32(x), _p(y), _isf32(y), _p(gamma), _p(beta), _p(mean), _p(rstd), T, D,
+    _lib.call("vj_layernorm_fwd", _p(x), _dtcode(x), _p(y), _dtcode(y), _p(gamma), _p(beta), _p(mean), _p(rstd), T, D,
               float(eps), _s())
     return y
 
@@ -122,13 +154,15 @@ def colsum(x, out, period=0, lo=0, hi=0):
 
 
 def im2col_tubelets(clips, patches, idx, tubelet, patch):
-    _chk(clips, F32, "clips"); _chk(patches, BF16, "patches")
+    """patches bf16, or fp16."""
+    name = _f16("vj_im2col_tubelets", patches)
+    _chk(clips, F32, "clips"); _chk(patches, None, "patches")
     B, C, T, H, W = clips.shape
     K = 0
     if idx is not None:
         _chk(idx, torch.int64, "idx")
         K = idx.shape[1]
-    _lib.call("vj_im2col_tubelets", _p(clips), _p(patches), _p(idx), B, C, T, H, W, tubelet, patch, K, _s())
+    _lib.call(name, _p(clips), _p(patches), _p(idx), B, C, T, H, W, tubelet, patch, K, _s())
     return patches
 
 
@@ -262,9 +296,15 @@ def cast_f32_bf16(src, dst):
     return dst
 
 
+def cast_f32_f16(src, dst):
+    _chk(src, F32, "src"); _chk(dst, F16, "dst")
+    _lib.call("vj_cast_f32_f16", _p(src), _p(dst), src.numel(), _s())
+    return dst
+
+
 def head_pad(src, dst, outer, G, hd, hdp, inner, unpad_add=False):
     _chk(src, None, "src"); _chk(dst, None, "dst")
-    _lib.call("vj_head_pad", _p(src), _isf32(src), _p(dst), _isf32(dst), outer, G, hd, hdp, inner, int(unpad_add), _s())
+    _lib.call("vj_head_pad", _p(src), _isf32(src), _p(dst), _dtcode(dst), outer, G, hd, hdp, inner, int(unpad_add), _s())
     return dst
 
 

@@ -125,8 +125,9 @@ def _common_base(tensors):
 # -------------------------------------------------------------------------------------------------
 class _EncoderFn(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, mod, clips, masks, final_norm, grid, *params):
-        save = any(ctx.needs_input_grad[5:])
+    def forward(ctx, mod, clips, masks, final_norm, grid, grad_enabled, *params):
+        # needs_input_grad follows requires_grad even under torch.no_grad(): a forward there keeps nothing for a backward
+        save = grad_enabled and any(ctx.needs_input_grad[6:])
         out, sv, _ = engine.encoder_forward(mod, clips, masks, save, final_norm=final_norm, grid=grid)
         if save and not final_norm:
             raise RuntimeError("training through the un-normalised encoder output is not supported")
@@ -139,7 +140,7 @@ class _EncoderFn(torch.autograd.Function):
         gflat = engine.encoder_backward(mod, sv, dout)
         ctx.sv = None
         grads = [sv.store.grad_view(gflat, n) if p.requires_grad else None for n, p in mod.named_parameters()]
-        return (None, None, None, None, None, *grads)
+        return (None, None, None, None, None, None, *grads)
 
 
 class _PredictorFn(torch.autograd.Function):
@@ -320,7 +321,7 @@ class VisionTransformer(nn.Module):
         """All masks in one fused pass.  Returns list of [B, K_i, D] bf16 views (one per mask)."""
         x, grid = self._check_input(x)
         params = [p for _, p in self.named_parameters()]
-        out = _EncoderFn.apply(self, x, list(masks), final_norm, grid, *params)
+        out = _EncoderFn.apply(self, x, list(masks), final_norm, grid, torch.is_grad_enabled(), *params)
         return _token_views(out, x.shape[0], [int(m.shape[1]) for m in masks])
 
     def forward(self, x, masks=None):
@@ -336,7 +337,7 @@ class VisionTransformer(nn.Module):
         if masks is None:
             xv, grid = self._check_input(x)
             params = [p for _, p in self.named_parameters()]
-            out = _EncoderFn.apply(self, xv, None, True, grid, *params)
+            out = _EncoderFn.apply(self, xv, None, True, grid, torch.is_grad_enabled(), *params)
             return out.view(xv.shape[0], grid[0] * grid[1] * grid[2], self.embed_dim)
         sizes = {int(m.shape[1]) for m in masks}
         if len(sizes) != 1:

@@ -32,6 +32,7 @@ class FlatParamStore:
     def __init__(self):
         self.flat = None      # fp32 [total]
         self.shadow = None    # bf16 [total]
+        self.shadow16 = None  # fp16 [total]: allocated by the first fp16 forward (evaluation under autocast(float16))
         self.offsets = {}     # name -> (offset, numel, shape)
         self.total = 0
         self._params = None
@@ -79,6 +80,7 @@ class FlatParamStore:
                 p._vj_store, p._vj_name = self, n
         self.flat, self.offsets, self.total, self._params = flat, offsets, off, named
         self.shadow = torch.empty(off, dtype=torch.bfloat16, device=dev)
+        self.shadow16 = None
         self._shadow_fresh = False
         self._shadow_complete = False
         self._seg = None
@@ -93,10 +95,17 @@ class FlatParamStore:
         return p.data_ptr() == self.flat.data_ptr() + 4 * off and tuple(p.shape) == shape
 
     # -- per-step products ---------------------------------------------------------------------
-    def refresh_shadow(self):
-        """bf16 operands of this forward.  The fused AdamW / EMA kernels already wrote them together with the parameter
-        update (one pass instead of update + cast); that copy is valid for exactly one refresh, anything else that may
-        have touched the parameters in between (load_state_dict, manual edits) is covered by casting again."""
+    def refresh_shadow(self, dtype=torch.bfloat16):
+        """bf16 (or fp16) operands of this forward.  The fused AdamW / EMA kernels already wrote the bf16 ones together
+        with the parameter update (one pass instead of update + cast); that copy is valid for exactly one refresh,
+        anything else that may have touched the parameters in between (load_state_dict, manual edits) is covered by
+        casting again.  Nothing writes the fp16 shadow but this cast, so an fp16 forward always casts, like a bf16 forward
+        of a network no optimizer updates."""
+        if dtype == torch.float16:
+            if self.shadow16 is None:
+                self.shadow16 = torch.empty(self.total, dtype=torch.float16, device=self.flat.device)
+            K.cast_f32_f16(self.flat, self.shadow16)
+            return
         if self._shadow_fresh:
             self._shadow_fresh = False
             return
@@ -130,6 +139,13 @@ class FlatParamStore:
     def bf16(self, name):
         o, n, shape = self.offsets[name]
         return self.shadow[o:o + n].view(shape)
+
+    def w16(self, name, dtype):
+        """Tensor-core operand of parameter `name` in `dtype`: the bf16 or the fp16 shadow."""
+        if dtype == torch.float16:
+            o, n, shape = self.offsets[name]
+            return self.shadow16[o:o + n].view(shape)
+        return self.bf16(name)
 
     def f32(self, name):
         o, n, shape = self.offsets[name]
