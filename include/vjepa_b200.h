@@ -50,8 +50,8 @@ long long vj_tmap_cache_stats(int which);
  * no epilogue): stream-K - the (tile, k-block) space is cut into one equal contiguous range per SM (weight gradients).
  * bias: fp32 [N] or NULL.  aux: bf16 or fp32 (aux_f32) tile source for ADD / MUL / DGELU.  An fp32 aux may be
  * row-mapped: row r reads aux row aux_rowmap[r] if given, else r % aux_period if aux_period > 0, else r (pos-embed
- * add of the patch-embed GEMM); a bf16 aux is a plain [M,N] matrix (residual stream / saved gelu') and does not
- * combine with split-K.  aux_out (bf16 [M,N], optional) is the second output of the GELU epilogues.
+ * add of the patch-embed GEMM); a bf16 aux is a plain [M,N] matrix (residual stream / saved gelu').  No aux epilogue
+ * combines with split-K (every piece runs the epilogue).  aux_out (bf16 [M,N], optional) is the second output of the GELU epilogues.
  * Replaces F.linear / Conv3d-as-GEMM and their backward:
  *   src/models/utils/modules.py:31-34,63,76; src/models/predictor.py:194,237;
  *   src/models/utils/patch_embed.py:54-57. */

@@ -760,11 +760,11 @@ static int gemm_impl(const void* A, long long lda, int a_mn, const void* B, long
   // aux_out is written by TMA stores: 16-byte aligned rows
   if (p.aux_out != nullptr)
     VJ_CHECK_ARG((reinterpret_cast<uintptr_t>(aux_out) & 15) == 0 && ldauxout % 8 == 0, "vj_gemm: aux_out misaligned");
-  const bool aux_tma = (epi == VJ_EPI_ADD || epi == VJ_EPI_DGELU || epi == VJ_EPI_MUL) && !aux_f32;
-  if (aux_tma) {
-    VJ_CHECK_ARG(aux_rowmap == nullptr && aux_period == 0, "vj_gemm: row-mapped / periodic aux must be fp32");
-    VJ_CHECK_ARG(p.split_k == 1, "vj_gemm: aux epilogues do not combine with split-K");
-  }
+  const bool uses_aux = epi == VJ_EPI_ADD || epi == VJ_EPI_DGELU || epi == VJ_EPI_MUL;
+  const bool aux_tma = uses_aux && !aux_f32;
+  // every split-K piece runs the whole epilogue: an fp32 aux would be added once per piece
+  if (uses_aux) VJ_CHECK_ARG(p.split_k == 1, "vj_gemm: aux epilogues do not combine with split-K");
+  if (aux_tma) VJ_CHECK_ARG(aux_rowmap == nullptr && aux_period == 0, "vj_gemm: row-mapped / periodic aux must be fp32");
   GemmMaps m;
   memset(&m, 0, sizeof(m));
   int rc;
