@@ -5,10 +5,11 @@ eval.py:63-521): a video encoder from pre-training sees each image repeated `fra
 reference :451-456), and the attentive probe trains on its tokens with one classifier call per step.  The optimizer,
 checkpoint and encoder-loading helpers are the video evaluation's (the reference has identical copies).
 
-The reference autocasts the loop to fp16 (eval.py:284).  This loop opens no autocast region, so encoder and probe compute
-bf16 x bf16 -> fp32, and `use_bfloat16` selects the GradScaler, as it does in the reference.  (Inside a caller's
-autocast(float16) the encoder would run its fp16 kernels and return fp32 features; the probe computes in bf16 either
-way.)
+The reference autocasts the loop body to fp16 (eval.py:284, `autocast(dtype=torch.float16, enabled=use_bfloat16)`).
+By default this loop opens no autocast region, so encoder and probe compute bf16 x bf16 -> fp32, and `use_bfloat16`
+selects the GradScaler, as it does in the reference.  `optimization.fp16_autocast: true` opens that region where the
+reference does and builds the classifier to follow it, exactly as in the video evaluation: fp16 encoder and probe with
+`use_bfloat16: true`, bf16 throughout with `use_bfloat16: false`.  There is no fp32 path.
 """
 import os
 
@@ -26,7 +27,8 @@ import torch
 import torch.multiprocessing as mp
 
 import src.models.vision_transformer as vit
-from evals.video_classification_frozen.eval import init_opt, load_checkpoint, load_pretrained, require_cuda
+from evals.video_classification_frozen.eval import (init_opt, load_checkpoint, load_pretrained, loop_autocast,
+                                                    read_fp16_autocast, require_cuda)
 from src.datasets.data_manager import init_data
 from src.models.attentive_pooler import AttentiveClassifier
 from src.utils.distributed import AllReduce, DistributedDataParallel, init_distributed
@@ -77,6 +79,7 @@ def main(args_eval, resume_preempt=False):
     final_lr = args_opt.get('final_lr')
     warmup = args_opt.get('warmup')
     use_bfloat16 = args_opt.get('use_bfloat16')
+    fp16_autocast = read_fp16_autocast(args_opt)
 
     resume_checkpoint = args_eval.get('resume_checkpoint', False) or resume_preempt
     eval_tag = args_eval.get('tag', None)
@@ -111,7 +114,7 @@ def main(args_eval, resume_preempt=False):
         p.requires_grad = False
 
     classifier = AttentiveClassifier(embed_dim=encoder.embed_dim, num_heads=encoder.num_heads, depth=1,
-                                     num_classes=num_classes).to(device)
+                                     num_classes=num_classes, follow_autocast=fp16_autocast).to(device)
 
     train_loader = make_dataloader(dataset_name=dataset_name, root_path=root_path, resolution=resolution,
                                    image_folder=image_folder, batch_size=batch_size, world_size=world_size, rank=rank,
@@ -152,10 +155,10 @@ def main(args_eval, resume_preempt=False):
         logger.info('Epoch %d' % (epoch + 1))
         train_acc = run_one_epoch(device=device, training=True, encoder=encoder, classifier=classifier, scaler=scaler,
                                   optimizer=optimizer, scheduler=scheduler, wd_scheduler=wd_scheduler,
-                                  data_loader=train_loader, use_bfloat16=use_bfloat16)
+                                  data_loader=train_loader, use_bfloat16=use_bfloat16, fp16_autocast=fp16_autocast)
         val_acc = run_one_epoch(device=device, training=False, encoder=encoder, classifier=classifier, scaler=scaler,
                                 optimizer=optimizer, scheduler=scheduler, wd_scheduler=wd_scheduler,
-                                data_loader=val_loader, use_bfloat16=use_bfloat16)
+                                data_loader=val_loader, use_bfloat16=use_bfloat16, fp16_autocast=fp16_autocast)
         logger.info('[%5d] train: %.3f%% test: %.3f%%' % (epoch + 1, train_acc, val_acc))
         if rank == 0:
             csv_logger.log(epoch + 1, train_acc, val_acc)
@@ -163,7 +166,7 @@ def main(args_eval, resume_preempt=False):
 
 
 def run_one_epoch(device, training, encoder, classifier, scaler, optimizer, scheduler, wd_scheduler, data_loader,
-                  use_bfloat16):
+                  use_bfloat16, fp16_autocast=False):
     """eval.py:262-317: one classifier call per step."""
     classifier.train(mode=training)
     criterion = torch.nn.CrossEntropyLoss()
@@ -174,18 +177,19 @@ def run_one_epoch(device, training, encoder, classifier, scaler, optimizer, sche
             scheduler.step()
             wd_scheduler.step()
 
-        # (no autocast region: encoder and probe compute bf16 x bf16 -> fp32; see the module docstring)
-        if isinstance(data[0], list):       # uint8 image tickets: the transform's pixel work runs on the GPU
-            imgs = data_loader.dataset.transform.batch(data[0], device)
-        else:
-            imgs = data[0].to(device)
-        labels = data[1].to(device)
-        with torch.no_grad():
-            outputs = encoder(imgs)
-            if not training:
+        # (without fp16_autocast no region: encoder and probe compute bf16 x bf16 -> fp32; see the module docstring)
+        with loop_autocast(fp16_autocast, use_bfloat16):
+            if isinstance(data[0], list):       # uint8 image tickets: the transform's pixel work runs on the GPU
+                imgs = data_loader.dataset.transform.batch(data[0], device)
+            else:
+                imgs = data[0].to(device)
+            labels = data[1].to(device)
+            with torch.no_grad():
+                outputs = encoder(imgs)
+                if not training:
+                    outputs = classifier(outputs)
+            if training:
                 outputs = classifier(outputs)
-        if training:
-            outputs = classifier(outputs)
 
         loss = criterion(outputs, labels)
         top1_acc = 100. * outputs.max(dim=1).indices.eq(labels).sum() / len(imgs)

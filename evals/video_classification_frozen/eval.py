@@ -9,11 +9,15 @@ eval.py:67-561), with every step on the sm_90a kernels of jepa_b200:
   DistributedDataParallel                           -> one averaging all-reduce of the probe's flat gradient per backward
   validation views (uint8 frames)                   -> vj_clip_views (EvalVideoTransform / VideoTransform eval path)
 
-The reference autocasts the loop to fp16 (eval.py:323).  This loop opens no autocast region, so encoder and probe compute
-bf16 x bf16 -> fp32, and `use_bfloat16` selects the GradScaler, as it does in the reference.  (Inside a caller's
-autocast(float16) the encoder would run its fp16 kernels and return fp32 features; the probe computes in bf16 either
-way.)
+The reference autocasts the loop body to fp16 (eval.py:323, `autocast(dtype=torch.float16, enabled=use_bfloat16)`).
+By default this loop opens no autocast region, so encoder and probe compute bf16 x bf16 -> fp32, and `use_bfloat16`
+selects the GradScaler, as it does in the reference.  With `optimization.fp16_autocast: true` the loop body runs inside
+that same region, where the reference opens it, and the classifier follows it (AttentiveClassifier(follow_autocast=True)):
+with `use_bfloat16: true` the encoder, the probe's forward and its backward compute in fp16 as the reference's do, with
+fp16 logits and GradScaler; with `use_bfloat16: false` the region is disabled, as in the reference, and everything
+computes in bf16 as by default.  There is no fp32 path.
 """
+import contextlib
 import os
 
 try:
@@ -100,6 +104,7 @@ def main(args_eval, resume_preempt=False):
     final_lr = args_opt.get('final_lr')
     warmup = args_opt.get('warmup')
     use_bfloat16 = args_opt.get('use_bfloat16')
+    fp16_autocast = read_fp16_autocast(args_opt)
 
     resume_checkpoint = args_eval.get('resume_checkpoint', False) or resume_preempt
     eval_tag = args_eval.get('tag', None)
@@ -145,7 +150,7 @@ def main(args_eval, resume_preempt=False):
         p.requires_grad = False
 
     classifier = AttentiveClassifier(embed_dim=encoder.embed_dim, num_heads=encoder.num_heads, depth=1,
-                                     num_classes=num_classes).to(device)
+                                     num_classes=num_classes, follow_autocast=fp16_autocast).to(device)
 
     train_loader = make_dataloader(dataset_type=dataset_type, root_path=train_data_path, resolution=resolution,
                                    frames_per_clip=eval_frames_per_clip, frame_step=eval_frame_step,
@@ -195,16 +200,34 @@ def main(args_eval, resume_preempt=False):
                                   num_temporal_views=eval_num_segments if attend_across_segments else 1,
                                   attend_across_segments=attend_across_segments, num_spatial_views=1, encoder=encoder,
                                   classifier=classifier, scaler=scaler, optimizer=optimizer, scheduler=scheduler,
-                                  wd_scheduler=wd_scheduler, data_loader=train_loader, use_bfloat16=use_bfloat16)
+                                  wd_scheduler=wd_scheduler, data_loader=train_loader, use_bfloat16=use_bfloat16,
+                                  fp16_autocast=fp16_autocast)
         val_acc = run_one_epoch(device=device, training=False, num_temporal_views=eval_num_segments,
                                 attend_across_segments=attend_across_segments,
                                 num_spatial_views=eval_num_views_per_segment, encoder=encoder, classifier=classifier,
                                 scaler=scaler, optimizer=optimizer, scheduler=scheduler, wd_scheduler=wd_scheduler,
-                                data_loader=val_loader, use_bfloat16=use_bfloat16)
+                                data_loader=val_loader, use_bfloat16=use_bfloat16, fp16_autocast=fp16_autocast)
         logger.info('[%5d] train: %.3f%% test: %.3f%%' % (epoch + 1, train_acc, val_acc))
         if rank == 0:
             csv_logger.log(epoch + 1, train_acc, val_acc)
         save_checkpoint(epoch + 1)
+
+
+def read_fp16_autocast(args_opt):
+    """`optimization.fp16_autocast` (default false): run the loop body inside the reference's
+    autocast(dtype=torch.float16, enabled=use_bfloat16) region, with a classifier that follows it."""
+    value = args_opt.get('fp16_autocast', False)
+    if not isinstance(value, bool):
+        raise ValueError(f"optimization.fp16_autocast must be true or false, got {value!r}")
+    return value
+
+
+def loop_autocast(fp16_autocast, use_bfloat16):
+    """The autocast region of one loop body: the reference's (eval.py:323) when fp16_autocast is set - disabled unless
+    use_bfloat16, as there - and none otherwise."""
+    if not fp16_autocast:
+        return contextlib.nullcontext()
+    return torch.autocast('cuda', dtype=torch.float16, enabled=bool(use_bfloat16))
 
 
 def load_clips(data, device, data_loader):
@@ -222,7 +245,7 @@ def load_clips(data, device, data_loader):
 
 
 def run_one_epoch(device, training, encoder, classifier, scaler, optimizer, scheduler, wd_scheduler, data_loader,
-                  use_bfloat16, num_spatial_views, num_temporal_views, attend_across_segments):
+                  use_bfloat16, num_spatial_views, num_temporal_views, attend_across_segments, fp16_autocast=False):
     """eval.py:298-380.  Without attend_across_segments every (view, segment) token set goes through the classifier on
     its own; the probe's backward adds all of them into one flat gradient buffer, exchanged once across ranks."""
     classifier.train(mode=training)
@@ -234,24 +257,25 @@ def run_one_epoch(device, training, encoder, classifier, scaler, optimizer, sche
             scheduler.step()
             wd_scheduler.step()
 
-        # (no autocast region: encoder and probe compute bf16 x bf16 -> fp32; see the module docstring)
-        clips = load_clips(data, device, data_loader)
-        clip_indices = [d.to(device, non_blocking=True) for d in data[2]]
-        labels = data[1].to(device)
-        batch_size = len(labels)
+        # (without fp16_autocast no region: encoder and probe compute bf16 x bf16 -> fp32; see the module docstring)
+        with loop_autocast(fp16_autocast, use_bfloat16):
+            clips = load_clips(data, device, data_loader)
+            clip_indices = [d.to(device, non_blocking=True) for d in data[2]]
+            labels = data[1].to(device)
+            batch_size = len(labels)
 
-        with torch.no_grad():
-            outputs = encoder(clips, clip_indices)
-            if not training:
+            with torch.no_grad():
+                outputs = encoder(clips, clip_indices)
+                if not training:
+                    if attend_across_segments:
+                        outputs = [classifier(o) for o in outputs]
+                    else:
+                        outputs = [[classifier(ost) for ost in os] for os in outputs]
+            if training:
                 if attend_across_segments:
                     outputs = [classifier(o) for o in outputs]
                 else:
                     outputs = [[classifier(ost) for ost in os] for os in outputs]
-        if training:
-            if attend_across_segments:
-                outputs = [classifier(o) for o in outputs]
-            else:
-                outputs = [[classifier(ost) for ost in os] for os in outputs]
 
         if attend_across_segments:
             loss = sum([criterion(o, labels) for o in outputs]) / len(outputs)

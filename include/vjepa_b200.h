@@ -102,11 +102,23 @@ size_t vj_layernorm_bwd_workspace(int T, int D);
 int vj_layernorm_bwd(const void* dy, const void* x, int x_f32, const float* gamma, const float* mean,
                      const float* rstd, const void* dres, void* dx, float* dgamma, float* dbeta,
                      void* workspace, size_t ws_bytes, int T, int D, void* stream);
+/* vj_layernorm_bwd with an fp16 dy [T,D] and fp32 x / dres / dx (workspace as vj_layernorm_bwd_workspace): the
+ * backward of the attentive probe's norm1 / norm2 (modules.py:172,174) under the evals' autocast(float16)
+ * (evals/video_classification_frozen/eval.py:323): LayerNorm reads the fp32 features / residual, and its gradient comes
+ * from the next fp16 Linear.  dgamma / dbeta fp32 [D] are accumulated (+=) in fp32. */
+int vj_layernorm_bwd_f16(const void* dy, const float* x, const float* gamma, const float* mean, const float* rstd,
+                         const float* dres, float* dx, float* dgamma, float* dbeta, void* workspace, size_t ws_bytes,
+                         int T, int D, void* stream);
 
 /* out[N] += column sums of in[T,N] (bf16|fp32) over rows r with lo <= r % period < hi (period<=0: all).
  * Bias gradients of every nn.Linear; mask-token gradient (predictor.py:207-210 backward). */
 int vj_colsum(const void* in, int in_f32, float* out, long long T, int N, long long ld, int period, int lo,
               int hi, void* stream);
+/* vj_colsum of fp16 rows (in fp16 [T,N], out fp32 [N] +=): the bias gradients of the attentive probe's kv, q, fc1 and
+ * fc2 Linears when the probe trains under the evals' autocast(float16) (evals/video_classification_frozen/eval.py:323,
+ * evals/image_classification_frozen/eval.py:284; backward of modules.py:31-34,138-153). */
+int vj_colsum_f16(const void* in, float* out, long long T, int N, long long ld, int period, int lo, int hi,
+                  void* stream);
 
 /* Tubelet im2col: clips fp32 [B,C,T,H,W] -> patches bf16 [B*K', C*tub*ps*ps] in Conv3d weight order
  * (c,dt,dh,dw); idx (int64 [B,K], nullable) gathers tokens first (context path), else K' = all tokens.
@@ -188,6 +200,18 @@ size_t vj_cross_attn_bwd_workspace(int B, int nq, int S, int H, int HD);
 int vj_cross_attn_bwd(const void* q, const void* kv, const void* out, const void* dout, const float* lse2, float* dq,
                       void* dkv, void* workspace, size_t ws_bytes, int B, int nq, int S, int H, int HD, float scale,
                       void* stream);
+/* The three above with fp16 q / kv / out / dout / dkv (lse2, dq and the workspace stay fp32; same workspace query,
+ * same key chunks and reduction order, still no atomics): CrossAttention's SDPA and its autograd under the evals'
+ * autocast(float16) (evals/video_classification_frozen/eval.py:323, evals/image_classification_frozen/eval.py:284),
+ * where the q / kv Linears emit fp16 and SDPA runs in fp16.  Every fp16 store rounds to nearest; a value past 65504
+ * becomes +-inf. */
+int vj_cross_attn_fwd_f16(const void* q, const void* kv, void* out, int B, int nq, int S, int H, int HD, float scale,
+                          void* stream);
+int vj_cross_attn_fwd_lse_f16(const void* q, const void* kv, void* out, float* lse2, int B, int nq, int S, int H, int HD,
+                              float scale, void* stream);
+int vj_cross_attn_bwd_f16(const void* q, const void* kv, const void* out, const void* dout, const float* lse2, float* dq,
+                          void* dkv, void* workspace, size_t ws_bytes, int B, int nq, int S, int H, int HD, float scale,
+                          void* stream);
 
 /* ---- flat-buffer parameter kernels ------------------------------------------------------------ */
 /* dst bf16[n] = src fp32[n]: the per-step bf16 shadow of the fp32 master weights (what autocast's

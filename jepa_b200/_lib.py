@@ -31,7 +31,9 @@ SIGNATURES = {
     "vj_layernorm_fwd": (I, [P, I, P, I, P, P, P, P, I, I, F, P]),
     "vj_layernorm_bwd_workspace": (Z, [I, I]),
     "vj_layernorm_bwd": (I, [P, P, I, P, P, P, P, P, P, P, P, Z, I, I, P]),
+    "vj_layernorm_bwd_f16": (I, [P, P, P, P, P, P, P, P, P, P, Z, I, I, P]),
     "vj_colsum": (I, [P, I, P, L, I, L, I, I, I, P]),
+    "vj_colsum_f16": (I, [P, P, L, I, L, I, I, I, P]),
     "vj_im2col_tubelets": (I, [P, P, P, I, I, I, I, I, I, I, I, P]),
     "vj_im2col_tubelets_f16": (I, [P, P, P, I, I, I, I, I, I, I, I, P]),
     "vj_pos_interp": (I, [P, P, I, I, I, I, I, I, I, c_double, c_double, c_double, I, P]),
@@ -50,6 +52,9 @@ SIGNATURES = {
     "vj_cross_attn_fwd_lse": (I, [P, P, P, P, I, I, I, I, I, F, P]),
     "vj_cross_attn_bwd_workspace": (Z, [I, I, I, I, I]),
     "vj_cross_attn_bwd": (I, [P, P, P, P, P, P, P, P, Z, I, I, I, I, I, F, P]),
+    "vj_cross_attn_fwd_f16": (I, [P, P, P, I, I, I, I, I, F, P]),
+    "vj_cross_attn_fwd_lse_f16": (I, [P, P, P, P, I, I, I, I, I, F, P]),
+    "vj_cross_attn_bwd_f16": (I, [P, P, P, P, P, P, P, P, Z, I, I, I, I, I, F, P]),
     "vj_token_std_bwd": (I, [P, P, P, F, P, I, I, I, F, F, P]),
     "vj_cast_f32_bf16": (I, [P, P, L, P]),
     "vj_cast_f32_f16": (I, [P, P, L, P]),

@@ -181,13 +181,17 @@ ln_fwd2_kernel(const __nv_bfloat16* __restrict__ x, __nv_bfloat16* __restrict__ 
 // dx = dres + rstd * (g*dy - mean(g*dy) - xhat * mean(g*dy*xhat)).  The row (x, dy) stays in registers in
 // its storage format between the two passes; dgamma/dbeta partial sums live in per-warp shared-memory
 // slices (no atomics, no persistent registers), reduced per block into [gridDim.x, D] partials.
-template <int NV, bool X_F32>
+// DY: the 16-bit type of dy - bf16, or fp16 with an fp32 x (the attentive probe's LayerNorms under the evals'
+// autocast(float16): fp32 inputs, fp16 gradients from the following fp16 Linear's dgrad).
+template <int NV, bool X_F32, typename DY = __nv_bfloat16>
 // (register caps chosen so nothing spills: with ~220 KB of the SM given to shared memory L1 is tiny and every
 // local-memory access is an L2 round trip)
 __global__ void __launch_bounds__(256, NV <= 2 ? 2 : 1)
-ln_bwd_kernel(const __nv_bfloat16* __restrict__ dy, const void* __restrict__ x, const float* __restrict__ gamma,
+ln_bwd_kernel(const DY* __restrict__ dy, const void* __restrict__ x, const float* __restrict__ gamma,
               const float* __restrict__ mean, const float* __restrict__ rstd, const void* __restrict__ dres,
               void* __restrict__ dx, float* __restrict__ part_dgamma, float* __restrict__ part_dbeta, int T, int D) {
+  static_assert(std::is_same<DY, __nv_bfloat16>::value || X_F32, "an fp16 dy pairs with an fp32 x only");
+  using E = Elt<DY>;
   extern __shared__ float sm[];  // [warps][2][D]
   const int lane = threadIdx.x & 31;
   const int wib = threadIdx.x >> 5;
@@ -223,8 +227,8 @@ ln_bwd_kernel(const __nv_bfloat16* __restrict__ dy, const void* __restrict__ x, 
           xf[4] = bf16_lo(xp[i].z); xf[5] = bf16_hi(xp[i].z); xf[6] = bf16_lo(xp[i].w); xf[7] = bf16_hi(xp[i].w);
         }
         dyp[i] = *reinterpret_cast<const uint4*>(dy + row * D + c * 8);
-        dyf[0] = bf16_lo(dyp[i].x); dyf[1] = bf16_hi(dyp[i].x); dyf[2] = bf16_lo(dyp[i].y); dyf[3] = bf16_hi(dyp[i].y);
-        dyf[4] = bf16_lo(dyp[i].z); dyf[5] = bf16_hi(dyp[i].z); dyf[6] = bf16_lo(dyp[i].w); dyf[7] = bf16_hi(dyp[i].w);
+        dyf[0] = E::lo(dyp[i].x); dyf[1] = E::hi(dyp[i].x); dyf[2] = E::lo(dyp[i].y); dyf[3] = E::hi(dyp[i].y);
+        dyf[4] = E::lo(dyp[i].z); dyf[5] = E::hi(dyp[i].z); dyf[6] = E::lo(dyp[i].w); dyf[7] = E::hi(dyp[i].w);
         ld8<true>(gamma, c * 8, g);
 #pragma unroll
         for (int j = 0; j < 8; ++j) {
@@ -248,8 +252,8 @@ ln_bwd_kernel(const __nv_bfloat16* __restrict__ dy, const void* __restrict__ x, 
           xf[0] = bf16_lo(xp[i].x); xf[1] = bf16_hi(xp[i].x); xf[2] = bf16_lo(xp[i].y); xf[3] = bf16_hi(xp[i].y);
           xf[4] = bf16_lo(xp[i].z); xf[5] = bf16_hi(xp[i].z); xf[6] = bf16_lo(xp[i].w); xf[7] = bf16_hi(xp[i].w);
         }
-        dyf[0] = bf16_lo(dyp[i].x); dyf[1] = bf16_hi(dyp[i].x); dyf[2] = bf16_lo(dyp[i].y); dyf[3] = bf16_hi(dyp[i].y);
-        dyf[4] = bf16_lo(dyp[i].z); dyf[5] = bf16_hi(dyp[i].z); dyf[6] = bf16_lo(dyp[i].w); dyf[7] = bf16_hi(dyp[i].w);
+        dyf[0] = E::lo(dyp[i].x); dyf[1] = E::hi(dyp[i].x); dyf[2] = E::lo(dyp[i].y); dyf[3] = E::hi(dyp[i].y);
+        dyf[4] = E::lo(dyp[i].z); dyf[5] = E::hi(dyp[i].z); dyf[6] = E::lo(dyp[i].w); dyf[7] = E::hi(dyp[i].w);
         ld8<true>(gamma, c * 8, g);
 #pragma unroll
         for (int j = 0; j < 8; ++j) {
@@ -517,6 +521,19 @@ static int launch_ln_bwd(const void* dy, const void* x, int x_f32, const float* 
   return grid;
 }
 
+template <int NV>
+static int launch_ln_bwd_f16(const __half* dy, const float* x, const float* gamma, const float* mean, const float* rstd,
+                             const float* dres, float* dx, float* pg, float* pb, int grid, int T, int D, cudaStream_t s) {
+  static bool configured = false;
+  if (!configured) {
+    cudaFuncSetAttribute(ln_bwd_kernel<NV, true, __half>, cudaFuncAttributeMaxDynamicSharedMemorySize, 8 * 2 * 2048 * 4);
+    configured = true;
+  }
+  ln_bwd_kernel<NV, true, __half><<<grid, 256, (size_t)8 * 2 * D * sizeof(float), s>>>(dy, x, gamma, mean, rstd, dres, dx,
+                                                                                       pg, pb, T, D);
+  return grid;
+}
+
 }  // namespace vj
 
 using namespace vj;
@@ -564,6 +581,33 @@ extern "C" int vj_layernorm_bwd(const void* dy, const void* x, int x_f32, const 
   float* pg = reinterpret_cast<float*>(workspace);
   float* pb = pg + (size_t)grid * D;
 #define VJ_CALL(NV) grid = launch_ln_bwd<NV>(dy, x, x_f32, gamma, mean, rstd, dres, dx, pg, pb, grid, T, D, s)
+  VJ_LN_DISPATCH(D, VJ_CALL);
+#undef VJ_CALL
+  VJ_CUDA(cudaGetLastError());
+  {
+    const int rows_per_block = 64;
+    dim3 rgrid((D + 31) / 32, (grid + rows_per_block - 1) / rows_per_block);
+    partial_reduce_kernel<<<rgrid, 256, 0, s>>>(pg, pb, dgamma, dbeta, grid, D, rows_per_block);
+  }
+  VJ_CUDA(cudaGetLastError());
+  vj::count_launch(2);
+  return 0;
+}
+
+extern "C" int vj_layernorm_bwd_f16(const void* dy, const float* x, const float* gamma, const float* mean,
+                                    const float* rstd, const float* dres, float* dx, float* dgamma, float* dbeta,
+                                    void* workspace, size_t ws_bytes, int T, int D, void* stream_) {
+  cudaStream_t s = reinterpret_cast<cudaStream_t>(stream_);
+  if (T <= 0) return 0;
+  VJ_CHECK_ARG(dy && x && gamma && mean && rstd && dx && dgamma && dbeta && workspace,
+               "vj_layernorm_bwd_f16: null pointer");
+  VJ_CHECK_ARG(D % 8 == 0 && D <= 2048, "vj_layernorm_bwd_f16: D=%d unsupported (multiple of 8, <= 2048)", D);
+  int grid = ln_bwd_grid(T);
+  VJ_CHECK_ARG(ws_bytes >= (size_t)grid * 2 * D * sizeof(float), "vj_layernorm_bwd_f16: workspace too small");
+  float* pg = reinterpret_cast<float*>(workspace);
+  float* pb = pg + (size_t)grid * D;
+  const __half* dyh = reinterpret_cast<const __half*>(dy);
+#define VJ_CALL(NV) grid = launch_ln_bwd_f16<NV>(dyh, x, gamma, mean, rstd, dres, dx, pg, pb, grid, T, D, s)
   VJ_LN_DISPATCH(D, VJ_CALL);
 #undef VJ_CALL
   VJ_CUDA(cudaGetLastError());

@@ -5,6 +5,8 @@
 #include "common.cuh"
 #include "vjepa_b200.h"
 
+#include <type_traits>
+
 namespace vj {
 
 constexpr int kMaxVec = 8;  // 8 chunks of 8 elements per lane -> D <= 2048
@@ -38,9 +40,10 @@ VJ_DEVINL void store8(void* base, long long elem_off, const float (&v)[8]) {
 
 // =============================================================================================
 // Column sum of a bf16 [T, N] matrix into fp32 out[N] (+=): bias gradients; with a periodic row
-// filter (rows r with lo <= r % period < hi) it is also the mask-token gradient.
+// filter (rows r with lo <= r % period < hi) it is also the mask-token gradient.  T16 is the 16-bit row
+// type when IN_F32 is false: bf16, or fp16 (the attentive probe's bias gradients under autocast(float16)).
 // =============================================================================================
-template <bool IN_F32>
+template <bool IN_F32, typename T16 = __nv_bfloat16>
 __global__ void __launch_bounds__(256) colsum_kernel(const void* __restrict__ in, float* __restrict__ out, long long T,
                                                      int N, long long ld, int rows_per_block, int period, int lo,
                                                      int hi) {
@@ -57,7 +60,14 @@ __global__ void __launch_bounds__(256) colsum_kernel(const void* __restrict__ in
         if (ph < lo || ph >= hi) continue;
       }
       float v[8];
-      load8<IN_F32>(in, r * ld + col, v);
+      if constexpr (IN_F32 || std::is_same<T16, __nv_bfloat16>::value) {
+        load8<IN_F32>(in, r * ld + col, v);
+      } else {
+        using E = Elt<T16>;
+        const uint4 u = *reinterpret_cast<const uint4*>(reinterpret_cast<const T16*>(in) + r * ld + col);
+        v[0] = E::lo(u.x); v[1] = E::hi(u.x); v[2] = E::lo(u.y); v[3] = E::hi(u.y);
+        v[4] = E::lo(u.z); v[5] = E::hi(u.z); v[6] = E::lo(u.w); v[7] = E::hi(u.w);
+      }
 #pragma unroll
       for (int j = 0; j < 8; ++j) acc[j] += v[j];
     }
@@ -471,11 +481,12 @@ static int grid_for(long long work_items, int per_block) {
 using namespace vj;
 
 
-extern "C" int vj_colsum(const void* in, int in_f32, float* out, long long T, int N, long long ld, int period, int lo,
-                         int hi, void* stream_) {
+// in_f32: 0 bf16, 1 fp32 (any non-zero value, as the ABI has always read it), 2 fp16 (vj_colsum_f16 only)
+static int colsum(const char* name, const void* in, int in_f32, float* out, long long T, int N, long long ld, int period,
+                  int lo, int hi, void* stream_) {
   cudaStream_t s = reinterpret_cast<cudaStream_t>(stream_);
-  VJ_CHECK_ARG(in && out, "vj_colsum: null pointer");
-  VJ_CHECK_ARG(N % 8 == 0 && ld % 8 == 0, "vj_colsum: N/ld must be multiples of 8");
+  VJ_CHECK_ARG(in && out, "%s: null pointer", name);
+  VJ_CHECK_ARG(N % 8 == 0 && ld % 8 == 0, "%s: N/ld must be multiples of 8", name);
   if (T <= 0) return 0;
   const int gx = (N + 255) / 256;
   long long want = (long long)num_sms() * 4 / gx;
@@ -484,11 +495,22 @@ extern "C" int vj_colsum(const void* in, int in_f32, float* out, long long T, in
   if (rpb < 64) rpb = 64;
   const int gy = int((T + rpb - 1) / rpb);
   dim3 grid(gx, gy);
-  if (in_f32) colsum_kernel<true><<<grid, 256, 0, s>>>(in, out, T, N, ld, int(rpb), period, lo, hi);
+  if (in_f32 == 2) colsum_kernel<false, __half><<<grid, 256, 0, s>>>(in, out, T, N, ld, int(rpb), period, lo, hi);
+  else if (in_f32) colsum_kernel<true><<<grid, 256, 0, s>>>(in, out, T, N, ld, int(rpb), period, lo, hi);
   else colsum_kernel<false><<<grid, 256, 0, s>>>(in, out, T, N, ld, int(rpb), period, lo, hi);
   VJ_CUDA(cudaGetLastError());
   vj::count_launch(1);
   return 0;
+}
+
+extern "C" int vj_colsum(const void* in, int in_f32, float* out, long long T, int N, long long ld, int period, int lo,
+                         int hi, void* stream) {
+  return colsum("vj_colsum", in, in_f32 ? 1 : 0, out, T, N, ld, period, lo, hi, stream);
+}
+
+extern "C" int vj_colsum_f16(const void* in, float* out, long long T, int N, long long ld, int period, int lo, int hi,
+                             void* stream) {
+  return colsum("vj_colsum_f16", in, 2, out, T, N, ld, period, lo, hi, stream);
 }
 
 template <typename TO>

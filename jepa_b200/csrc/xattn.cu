@@ -5,6 +5,8 @@
 //   q   bf16 [B*nq, H*hd]          (the q Linear's output; row b*nq + j = query j of clip b)
 //   kv  bf16 [B*S, 2*H*hd]         (the kv Linear's output: k | v halves, head-major inside a half)
 //   out bf16 [B*nq, H*hd] = softmax(q k^T * scale) v      per (clip, head, query)
+// The _f16 entry points run the same kernels on fp16 q / kv / out / dout / dkv (the probe under the evals'
+// autocast(float16)); lse2, dq and the dq partials stay fp32 either way.
 //
 // nq is 1 for the probe, S is 1568 .. 9216 encoder tokens: the work is a GEMV-shaped streaming pass over K and V
 // (2 * S * hd * 2 bytes per (clip, head)), i.e. HBM / L2 bound, so there is nothing for the tensor cores to do: one CTA per
@@ -22,16 +24,24 @@
 #include "common.cuh"
 #include "vjepa_b200.h"
 
+#include <type_traits>
+
 namespace vj {
 
 constexpr int kXattnThreads = 256;
 
-template <int LPK>   // lanes per key = hd / 8
-__global__ void __launch_bounds__(kXattnThreads) xattn_fwd_kernel(const __nv_bfloat16* __restrict__ q,
-                                                                  const __nv_bfloat16* __restrict__ kv,
-                                                                  __nv_bfloat16* __restrict__ out,
-                                                                  float* __restrict__ lse2, int nq, int S, int H,
-                                                                  float scale_log2) {
+// one 16-bit element of T from fp32, rounded to nearest (fp16: a value past 65504 becomes +-inf, never saturates)
+template <typename T>
+VJ_DEVINL T to_elt(float v) {
+  if constexpr (std::is_same<T, __half>::value) return __float2half_rn(v);
+  else return __float2bfloat16(v);
+}
+
+template <typename T, int LPK>   // T: bf16 or fp16 element type of q / kv / out; lanes per key = hd / 8
+__global__ void __launch_bounds__(kXattnThreads) xattn_fwd_kernel(const T* __restrict__ q, const T* __restrict__ kv,
+                                                                  T* __restrict__ out, float* __restrict__ lse2, int nq,
+                                                                  int S, int H, float scale_log2) {
+  using E = Elt<T>;
   constexpr int HD = LPK * 8;
   constexpr int KPW = 32 / LPK;                 // keys handled per warp iteration
   constexpr int NGROUPS = (kXattnThreads / 32) * KPW;
@@ -45,13 +55,13 @@ __global__ void __launch_bounds__(kXattnThreads) xattn_fwd_kernel(const __nv_bfl
   float qf[8];
   {
     const uint4 u = *reinterpret_cast<const uint4*>(q + (long long)bq * D + head * HD + (active ? gl : 0) * 8);
-    qf[0] = bf16_lo(u.x); qf[1] = bf16_hi(u.x); qf[2] = bf16_lo(u.y); qf[3] = bf16_hi(u.y);
-    qf[4] = bf16_lo(u.z); qf[5] = bf16_hi(u.z); qf[6] = bf16_lo(u.w); qf[7] = bf16_hi(u.w);
+    qf[0] = E::lo(u.x); qf[1] = E::hi(u.x); qf[2] = E::lo(u.y); qf[3] = E::hi(u.y);
+    qf[4] = E::lo(u.z); qf[5] = E::hi(u.z); qf[6] = E::lo(u.w); qf[7] = E::hi(u.w);
   }
   float m = -INFINITY, l = 0.f, o[8];
 #pragma unroll
   for (int i = 0; i < 8; ++i) o[i] = 0.f;
-  const __nv_bfloat16* kbase = kv + (long long)b * S * 2 * D + head * HD + gl * 8;
+  const T* kbase = kv + (long long)b * S * 2 * D + head * HD + gl * 8;
   for (int j0 = warp * KPW; j0 < S; j0 += (kXattnThreads / 32) * KPW) {
     const int j = j0 + grp;
     const bool ok = active && j < S;
@@ -60,8 +70,8 @@ __global__ void __launch_bounds__(kXattnThreads) xattn_fwd_kernel(const __nv_bfl
     if (ok) {
       const uint4 ku = *reinterpret_cast<const uint4*>(kbase + (long long)j * 2 * D);
       vv = *reinterpret_cast<const uint4*>(kbase + (long long)j * 2 * D + D);
-      part = qf[0] * bf16_lo(ku.x) + qf[1] * bf16_hi(ku.x) + qf[2] * bf16_lo(ku.y) + qf[3] * bf16_hi(ku.y) +
-             qf[4] * bf16_lo(ku.z) + qf[5] * bf16_hi(ku.z) + qf[6] * bf16_lo(ku.w) + qf[7] * bf16_hi(ku.w);
+      part = qf[0] * E::lo(ku.x) + qf[1] * E::hi(ku.x) + qf[2] * E::lo(ku.y) + qf[3] * E::hi(ku.y) +
+             qf[4] * E::lo(ku.z) + qf[5] * E::hi(ku.z) + qf[6] * E::lo(ku.w) + qf[7] * E::hi(ku.w);
     }
     // score of key j = sum of the LPK partial dot products of its lane group (rotation inside the group)
     float s = part;
@@ -73,10 +83,10 @@ __global__ void __launch_bounds__(kXattnThreads) xattn_fwd_kernel(const __nv_bfl
       const float corr = ex2_approx(m - mn);      // 0 on the first key (m = -inf)
       const float p = ex2_approx(s - mn);
       l = l * corr + p;
-      o[0] = o[0] * corr + p * bf16_lo(vv.x); o[1] = o[1] * corr + p * bf16_hi(vv.x);
-      o[2] = o[2] * corr + p * bf16_lo(vv.y); o[3] = o[3] * corr + p * bf16_hi(vv.y);
-      o[4] = o[4] * corr + p * bf16_lo(vv.z); o[5] = o[5] * corr + p * bf16_hi(vv.z);
-      o[6] = o[6] * corr + p * bf16_lo(vv.w); o[7] = o[7] * corr + p * bf16_hi(vv.w);
+      o[0] = o[0] * corr + p * E::lo(vv.x); o[1] = o[1] * corr + p * E::hi(vv.x);
+      o[2] = o[2] * corr + p * E::lo(vv.y); o[3] = o[3] * corr + p * E::hi(vv.y);
+      o[4] = o[4] * corr + p * E::lo(vv.z); o[5] = o[5] * corr + p * E::hi(vv.z);
+      o[6] = o[6] * corr + p * E::lo(vv.w); o[7] = o[7] * corr + p * E::hi(vv.w);
       m = mn;
     }
   }
@@ -99,7 +109,7 @@ __global__ void __launch_bounds__(kXattnThreads) xattn_fwd_kernel(const __nv_bfl
       L += w * sm_l[g];
       acc += w * sm_o[g][d];
     }
-    out[(long long)bq * D + head * HD + d] = __float2bfloat16(acc / L);
+    out[(long long)bq * D + head * HD + d] = to_elt<T>(acc / L);
     if (lse2 != nullptr && d == 0) lse2[(long long)bq * H + head] = M + log2f(L);
   }
 }
@@ -121,14 +131,18 @@ VJ_DEVINL float group_sum(float v) {
   }
 }
 
+template <typename T>
 VJ_DEVINL void unpack8(const uint4& u, float* f) {
-  f[0] = bf16_lo(u.x); f[1] = bf16_hi(u.x); f[2] = bf16_lo(u.y); f[3] = bf16_hi(u.y);
-  f[4] = bf16_lo(u.z); f[5] = bf16_hi(u.z); f[6] = bf16_lo(u.w); f[7] = bf16_hi(u.w);
+  using E = Elt<T>;
+  f[0] = E::lo(u.x); f[1] = E::hi(u.x); f[2] = E::lo(u.y); f[3] = E::hi(u.y);
+  f[4] = E::lo(u.z); f[5] = E::hi(u.z); f[6] = E::lo(u.w); f[7] = E::hi(u.w);
 }
 
+template <typename T>
 VJ_DEVINL float dot8(const float* a, const uint4& u) {
-  return a[0] * bf16_lo(u.x) + a[1] * bf16_hi(u.x) + a[2] * bf16_lo(u.y) + a[3] * bf16_hi(u.y) +
-         a[4] * bf16_lo(u.z) + a[5] * bf16_hi(u.z) + a[6] * bf16_lo(u.w) + a[7] * bf16_hi(u.w);
+  using E = Elt<T>;
+  return a[0] * E::lo(u.x) + a[1] * E::hi(u.x) + a[2] * E::lo(u.y) + a[3] * E::hi(u.y) +
+         a[4] * E::lo(u.z) + a[5] * E::hi(u.z) + a[6] * E::lo(u.w) + a[7] * E::hi(u.w);
 }
 
 constexpr int kXattnBwdKeys = 2;   // keys per lane group per CTA, held in registers from the first load to the store
@@ -139,11 +153,12 @@ __host__ __device__ constexpr int xattn_bwd_chunk() { return (kXattnThreads / 32
 // grid (H, B, key chunks).  Lane group g of the CTA owns keys chunk*KPC + kk*NGROUPS + g, kk < kXattnBwdKeys, so
 // consecutive groups read consecutive kv rows.  All nq queries of the clip are applied to those keys one after the other;
 // the per-query dq partial of the chunk is reduced over the groups through shared memory in group order.
-template <int LPK>
+template <typename T, int LPK>
 __global__ void __launch_bounds__(kXattnThreads, 2) xattn_bwd_kernel(
-    const __nv_bfloat16* __restrict__ q, const __nv_bfloat16* __restrict__ kv, const __nv_bfloat16* __restrict__ out,
-    const __nv_bfloat16* __restrict__ dout, const float* __restrict__ lse2, __nv_bfloat16* __restrict__ dkv,
-    float* __restrict__ dq_part, int nq, int S, int H, float scale_log2, float scale) {
+    const T* __restrict__ q, const T* __restrict__ kv, const T* __restrict__ out, const T* __restrict__ dout,
+    const float* __restrict__ lse2, T* __restrict__ dkv, float* __restrict__ dq_part, int nq, int S, int H,
+    float scale_log2, float scale) {
+  using E = Elt<T>;
   constexpr int HD = LPK * 8;
   constexpr int KPW = 32 / LPK;
   constexpr int NGROUPS = (kXattnThreads / 32) * KPW;
@@ -180,9 +195,9 @@ __global__ void __launch_bounds__(kXattnThreads, 2) xattn_bwd_kernel(
     const long long row = (long long)b * nq + i;
     const long long c = row * D + head * HD + (active ? gl : 0) * 8;
     float qf[8], df[8], of[8];
-    unpack8(*reinterpret_cast<const uint4*>(q + c), qf);
-    unpack8(*reinterpret_cast<const uint4*>(dout + c), df);
-    unpack8(*reinterpret_cast<const uint4*>(out + c), of);
+    unpack8<T>(*reinterpret_cast<const uint4*>(q + c), qf);
+    unpack8<T>(*reinterpret_cast<const uint4*>(dout + c), df);
+    unpack8<T>(*reinterpret_cast<const uint4*>(out + c), of);
     float dpart = 0.f;
 #pragma unroll
     for (int e = 0; e < 8; ++e) dpart += df[e] * of[e];
@@ -193,13 +208,13 @@ __global__ void __launch_bounds__(kXattnThreads, 2) xattn_bwd_kernel(
     for (int e = 0; e < 8; ++e) dqa[e] = 0.f;
 #pragma unroll
     for (int kk = 0; kk < NK; ++kk) {
-      const float s = group_sum<LPK>(dot8(qf, ku[kk]));
-      const float dp = group_sum<LPK>(dot8(df, vu[kk]));
+      const float s = group_sum<LPK>(dot8<T>(qf, ku[kk]));
+      const float dp = group_sum<LPK>(dot8<T>(df, vu[kk]));
       if (ok[kk]) {
         const float p = ex2_approx(s * scale_log2 - lse);
         const float ds = p * (dp - delta);
         float kf[8];
-        unpack8(ku[kk], kf);
+        unpack8<T>(ku[kk], kf);
 #pragma unroll
         for (int e = 0; e < 8; ++e) {
           dk[kk][e] += ds * qf[e];
@@ -225,10 +240,10 @@ __global__ void __launch_bounds__(kXattnThreads, 2) xattn_bwd_kernel(
     if (!ok[kk]) continue;
     const int j = chunk * KPC + kk * NGROUPS + g;
     uint4 a, v;
-    a.x = pack_bf16x2(dk[kk][0] * scale, dk[kk][1] * scale); a.y = pack_bf16x2(dk[kk][2] * scale, dk[kk][3] * scale);
-    a.z = pack_bf16x2(dk[kk][4] * scale, dk[kk][5] * scale); a.w = pack_bf16x2(dk[kk][6] * scale, dk[kk][7] * scale);
-    v.x = pack_bf16x2(dv[kk][0], dv[kk][1]); v.y = pack_bf16x2(dv[kk][2], dv[kk][3]);
-    v.z = pack_bf16x2(dv[kk][4], dv[kk][5]); v.w = pack_bf16x2(dv[kk][6], dv[kk][7]);
+    a.x = E::pack(dk[kk][0] * scale, dk[kk][1] * scale); a.y = E::pack(dk[kk][2] * scale, dk[kk][3] * scale);
+    a.z = E::pack(dk[kk][4] * scale, dk[kk][5] * scale); a.w = E::pack(dk[kk][6] * scale, dk[kk][7] * scale);
+    v.x = E::pack(dv[kk][0], dv[kk][1]); v.y = E::pack(dv[kk][2], dv[kk][3]);
+    v.z = E::pack(dv[kk][4], dv[kk][5]); v.w = E::pack(dv[kk][6], dv[kk][7]);
     *reinterpret_cast<uint4*>(dkv + kvoff + (long long)j * 2 * D) = a;
     *reinterpret_cast<uint4*>(dkv + kvoff + (long long)j * 2 * D + D) = v;
   }
@@ -260,25 +275,25 @@ static int xattn_bwd_chunks(int S, int HD) {
 
 using namespace vj;
 
-static int cross_attn_fwd(const void* q, const void* kv, void* out, float* lse2, int B, int nq, int S, int H, int HD,
-                          float scale, void* stream_) {
+template <typename T>
+static int cross_attn_fwd(const char* name, const void* q, const void* kv, void* out, float* lse2, int B, int nq, int S,
+                          int H, int HD, float scale, void* stream_) {
   cudaStream_t s = reinterpret_cast<cudaStream_t>(stream_);
-  VJ_CHECK_ARG(q && kv && out, "vj_cross_attn_fwd: null pointer");
-  VJ_CHECK_ARG(B > 0 && nq > 0 && S > 0 && H > 0, "vj_cross_attn_fwd: empty problem");
+  VJ_CHECK_ARG(q && kv && out, "%s: null pointer", name);
+  VJ_CHECK_ARG(B > 0 && nq > 0 && S > 0 && H > 0, "%s: empty problem", name);
   VJ_CHECK_ARG((reinterpret_cast<uintptr_t>(q) & 15) == 0 && (reinterpret_cast<uintptr_t>(kv) & 15) == 0,
-               "vj_cross_attn_fwd: pointers must be 16-byte aligned");
+               "%s: pointers must be 16-byte aligned", name);
   dim3 grid(H, B * nq);
   const float sl2 = scale * 1.4426950408889634f;
 #define VJ_XATTN(LPK)                                                                                                    \
-  xattn_fwd_kernel<LPK><<<grid, kXattnThreads, 0, s>>>(reinterpret_cast<const __nv_bfloat16*>(q),                        \
-                                                       reinterpret_cast<const __nv_bfloat16*>(kv),                       \
-                                                       reinterpret_cast<__nv_bfloat16*>(out), lse2, nq, S, H, sl2)
+  xattn_fwd_kernel<T, LPK><<<grid, kXattnThreads, 0, s>>>(reinterpret_cast<const T*>(q), reinterpret_cast<const T*>(kv), \
+                                                          reinterpret_cast<T*>(out), lse2, nq, S, H, sl2)
   switch (HD) {
     case 32: VJ_XATTN(4); break;
     case 64: VJ_XATTN(8); break;
     case 80: VJ_XATTN(10); break;
     case 128: VJ_XATTN(16); break;
-    default: set_error("vj_cross_attn_fwd: head dim %d unsupported (32 / 64 / 80 / 128)", HD); return -1;
+    default: set_error("%s: head dim %d unsupported (32 / 64 / 80 / 128)", name, HD); return -1;
   }
 #undef VJ_XATTN
   VJ_CUDA(cudaGetLastError());
@@ -288,13 +303,24 @@ static int cross_attn_fwd(const void* q, const void* kv, void* out, float* lse2,
 
 extern "C" int vj_cross_attn_fwd(const void* q, const void* kv, void* out, int B, int nq, int S, int H, int HD, float scale,
                                  void* stream) {
-  return cross_attn_fwd(q, kv, out, nullptr, B, nq, S, H, HD, scale, stream);
+  return cross_attn_fwd<__nv_bfloat16>("vj_cross_attn_fwd", q, kv, out, nullptr, B, nq, S, H, HD, scale, stream);
 }
 
 extern "C" int vj_cross_attn_fwd_lse(const void* q, const void* kv, void* out, float* lse2, int B, int nq, int S, int H,
                                      int HD, float scale, void* stream) {
   VJ_CHECK_ARG(lse2, "vj_cross_attn_fwd_lse: null lse2");
-  return cross_attn_fwd(q, kv, out, lse2, B, nq, S, H, HD, scale, stream);
+  return cross_attn_fwd<__nv_bfloat16>("vj_cross_attn_fwd_lse", q, kv, out, lse2, B, nq, S, H, HD, scale, stream);
+}
+
+extern "C" int vj_cross_attn_fwd_f16(const void* q, const void* kv, void* out, int B, int nq, int S, int H, int HD,
+                                     float scale, void* stream) {
+  return cross_attn_fwd<__half>("vj_cross_attn_fwd_f16", q, kv, out, nullptr, B, nq, S, H, HD, scale, stream);
+}
+
+extern "C" int vj_cross_attn_fwd_lse_f16(const void* q, const void* kv, void* out, float* lse2, int B, int nq, int S,
+                                         int H, int HD, float scale, void* stream) {
+  VJ_CHECK_ARG(lse2, "vj_cross_attn_fwd_lse_f16: null lse2");
+  return cross_attn_fwd<__half>("vj_cross_attn_fwd_lse_f16", q, kv, out, lse2, B, nq, S, H, HD, scale, stream);
 }
 
 extern "C" size_t vj_cross_attn_bwd_workspace(int B, int nq, int S, int H, int HD) {
@@ -303,27 +329,27 @@ extern "C" size_t vj_cross_attn_bwd_workspace(int B, int nq, int S, int H, int H
   return (size_t)nchunk * B * nq * H * HD * sizeof(float);
 }
 
-extern "C" int vj_cross_attn_bwd(const void* q, const void* kv, const void* out, const void* dout, const float* lse2,
-                                 float* dq, void* dkv, void* workspace, size_t ws_bytes, int B, int nq, int S, int H, int HD,
-                                 float scale, void* stream_) {
+template <typename T>
+static int cross_attn_bwd(const char* name, const void* q, const void* kv, const void* out, const void* dout,
+                          const float* lse2, float* dq, void* dkv, void* workspace, size_t ws_bytes, int B, int nq, int S,
+                          int H, int HD, float scale, void* stream_) {
   cudaStream_t s = reinterpret_cast<cudaStream_t>(stream_);
-  VJ_CHECK_ARG(q && kv && out && dout && lse2 && dq && dkv && workspace, "vj_cross_attn_bwd: null pointer");
-  VJ_CHECK_ARG(B > 0 && nq > 0 && S > 0 && H > 0, "vj_cross_attn_bwd: empty problem");
+  VJ_CHECK_ARG(q && kv && out && dout && lse2 && dq && dkv && workspace, "%s: null pointer", name);
+  VJ_CHECK_ARG(B > 0 && nq > 0 && S > 0 && H > 0, "%s: empty problem", name);
   const int nchunk = xattn_bwd_chunks(S, HD);
-  VJ_CHECK_ARG(nchunk > 0, "vj_cross_attn_bwd: head dim %d unsupported (32 / 64 / 80 / 128)", HD);
-  VJ_CHECK_ARG(nchunk <= 65535, "vj_cross_attn_bwd: S = %d keys is too long", S);
-  VJ_CHECK_ARG(ws_bytes >= vj_cross_attn_bwd_workspace(B, nq, S, H, HD), "vj_cross_attn_bwd: workspace too small");
+  VJ_CHECK_ARG(nchunk > 0, "%s: head dim %d unsupported (32 / 64 / 80 / 128)", name, HD);
+  VJ_CHECK_ARG(nchunk <= 65535, "%s: S = %d keys is too long", name, S);
+  VJ_CHECK_ARG(ws_bytes >= vj_cross_attn_bwd_workspace(B, nq, S, H, HD), "%s: workspace too small", name);
   VJ_CHECK_ARG(((reinterpret_cast<uintptr_t>(q) | reinterpret_cast<uintptr_t>(kv) | reinterpret_cast<uintptr_t>(out) |
                  reinterpret_cast<uintptr_t>(dout) | reinterpret_cast<uintptr_t>(dkv)) & 15) == 0,
-               "vj_cross_attn_bwd: pointers must be 16-byte aligned");
+               "%s: pointers must be 16-byte aligned", name);
   dim3 grid(H, B, nchunk);
   const float sl2 = scale * 1.4426950408889634f;
   float* part = reinterpret_cast<float*>(workspace);
 #define VJ_XATTN_BWD(LPK)                                                                                              \
-  xattn_bwd_kernel<LPK><<<grid, kXattnThreads, 0, s>>>(                                                                \
-      reinterpret_cast<const __nv_bfloat16*>(q), reinterpret_cast<const __nv_bfloat16*>(kv),                          \
-      reinterpret_cast<const __nv_bfloat16*>(out), reinterpret_cast<const __nv_bfloat16*>(dout), lse2,                \
-      reinterpret_cast<__nv_bfloat16*>(dkv), part, nq, S, H, sl2, scale)
+  xattn_bwd_kernel<T, LPK><<<grid, kXattnThreads, 0, s>>>(                                                             \
+      reinterpret_cast<const T*>(q), reinterpret_cast<const T*>(kv), reinterpret_cast<const T*>(out),                  \
+      reinterpret_cast<const T*>(dout), lse2, reinterpret_cast<T*>(dkv), part, nq, S, H, sl2, scale)
   switch (HD) {
     case 32: VJ_XATTN_BWD(4); break;
     case 64: VJ_XATTN_BWD(8); break;
@@ -338,4 +364,18 @@ extern "C" int vj_cross_attn_bwd(const void* q, const void* kv, const void* out,
   VJ_CUDA(cudaGetLastError());
   vj::count_launch(2);
   return 0;
+}
+
+extern "C" int vj_cross_attn_bwd(const void* q, const void* kv, const void* out, const void* dout, const float* lse2,
+                                 float* dq, void* dkv, void* workspace, size_t ws_bytes, int B, int nq, int S, int H, int HD,
+                                 float scale, void* stream) {
+  return cross_attn_bwd<__nv_bfloat16>("vj_cross_attn_bwd", q, kv, out, dout, lse2, dq, dkv, workspace, ws_bytes, B, nq,
+                                       S, H, HD, scale, stream);
+}
+
+extern "C" int vj_cross_attn_bwd_f16(const void* q, const void* kv, const void* out, const void* dout, const float* lse2,
+                                     float* dq, void* dkv, void* workspace, size_t ws_bytes, int B, int nq, int S, int H,
+                                     int HD, float scale, void* stream) {
+  return cross_attn_bwd<__half>("vj_cross_attn_bwd_f16", q, kv, out, dout, lse2, dq, dkv, workspace, ws_bytes, B, nq, S,
+                                H, HD, scale, stream);
 }

@@ -132,8 +132,15 @@ _ln_ws = {}
 
 
 def layernorm_bwd(dy, x, gamma, mean, rstd, dres, dx, dgamma, dbeta):
-    _chk(dy, BF16, "dy"); _chk(x, None, "x"); _chk(dx, x.dtype, "dx")
+    """dy bf16 with x / dres / dx bf16 or fp32; or dy fp16 with x / dres / dx fp32 (vj_layernorm_bwd_f16)."""
+    _chk(dy, None, "dy"); _chk(x, None, "x"); _chk(dx, x.dtype, "dx")
     _chk(dgamma, F32, "dgamma"); _chk(dbeta, F32, "dbeta")
+    if dy.dtype == F16:
+        _chk(x, F32, "x (with an fp16 dy)")
+        if dres is not None:
+            _chk(dres, F32, "dres (with an fp16 dy)")
+    elif dy.dtype != BF16:
+        raise _lib.VJError(f"layernorm_bwd: dy must be bf16 or fp16, got {dy.dtype}")
     T, D = x.shape
     need = _lib.load().vj_layernorm_bwd_workspace(T, D)
     key = (x.device.index, torch.cuda.current_stream().cuda_stream)
@@ -141,15 +148,23 @@ def layernorm_bwd(dy, x, gamma, mean, rstd, dres, dx, dgamma, dbeta):
     if ws is None or ws.numel() < need:
         ws = torch.empty(need, dtype=torch.uint8, device=x.device)
         _ln_ws[key] = ws
-    _lib.call("vj_layernorm_bwd", _p(dy), _p(x), _isf32(x), _p(gamma), _p(mean), _p(rstd), _p(dres), _p(dx),
-              _p(dgamma), _p(dbeta), _p(ws), ws.numel(), T, D, _s())
+    if dy.dtype == F16:
+        _lib.call("vj_layernorm_bwd_f16", _p(dy), _p(x), _p(gamma), _p(mean), _p(rstd), _p(dres), _p(dx), _p(dgamma),
+                  _p(dbeta), _p(ws), ws.numel(), T, D, _s())
+    else:
+        _lib.call("vj_layernorm_bwd", _p(dy), _p(x), _isf32(x), _p(gamma), _p(mean), _p(rstd), _p(dres), _p(dx),
+                  _p(dgamma), _p(dbeta), _p(ws), ws.numel(), T, D, _s())
     return dx
 
 
 def colsum(x, out, period=0, lo=0, hi=0):
+    """out[N] += column sums of x [T, N] (bf16, fp16 or fp32) over rows r with lo <= r % period < hi."""
     _chk(x, None, "x"); _chk(out, F32, "out")
     T, N = x.shape
-    _lib.call("vj_colsum", _p(x), _isf32(x), _p(out), T, N, x.stride(0), period, lo, hi, _s())
+    if x.dtype == F16:
+        _lib.call("vj_colsum_f16", _p(x), _p(out), T, N, x.stride(0), period, lo, hi, _s())
+    else:
+        _lib.call("vj_colsum", _p(x), _isf32(x), _p(out), T, N, x.stride(0), period, lo, hi, _s())
     return out
 
 
@@ -259,27 +274,32 @@ def token_std_bwd(z, pstd_total, grad_scale, scale, dz, weight, eps=1e-4):
 
 
 def cross_attn_fwd(q, kv, out, B, nq, S, H, hd, scale):
-    """softmax(q k^T scale) v for nq query tokens per clip over S keys (attentive probe, modules.py:138-153)."""
-    _chk(q, BF16, "q"); _chk(kv, BF16, "kv"); _chk(out, BF16, "out")
-    _lib.call("vj_cross_attn_fwd", _p(q), _p(kv), _p(out), B, nq, S, H, hd, float(scale), _s())
+    """softmax(q k^T scale) v for nq query tokens per clip over S keys (attentive probe, modules.py:138-153).
+    q, kv and out are all bf16 or all fp16."""
+    name = _f16("vj_cross_attn_fwd", q)
+    _chk(q, None, "q"); _chk(kv, q.dtype, "kv"); _chk(out, q.dtype, "out")
+    _lib.call(name, _p(q), _p(kv), _p(out), B, nq, S, H, hd, float(scale), _s())
     return out
 
 
 def cross_attn_fwd_lse(q, kv, out, lse2, B, nq, S, H, hd, scale):
     """cross_attn_fwd that also writes the softmax statistics lse2 fp32 [B*nq, H] (log2 domain) for the backward."""
-    _chk(q, BF16, "q"); _chk(kv, BF16, "kv"); _chk(out, BF16, "out"); _chk(lse2, F32, "lse2")
-    _lib.call("vj_cross_attn_fwd_lse", _p(q), _p(kv), _p(out), _p(lse2), B, nq, S, H, hd, float(scale), _s())
+    name = _f16("vj_cross_attn_fwd_lse", q)
+    _chk(q, None, "q"); _chk(kv, q.dtype, "kv"); _chk(out, q.dtype, "out"); _chk(lse2, F32, "lse2")
+    _lib.call(name, _p(q), _p(kv), _p(out), _p(lse2), B, nq, S, H, hd, float(scale), _s())
     return out
 
 
 def cross_attn_bwd(q, kv, out, dout, lse2, dq, dkv, B, nq, S, H, hd, scale):
-    """dq fp32 [B*nq, H*hd] and dkv bf16 [B*S, 2*H*hd] of cross_attn_fwd_lse."""
+    """dq fp32 [B*nq, H*hd] and dkv [B*S, 2*H*hd] of cross_attn_fwd_lse; q, kv, out, dout and dkv are all bf16 or all
+    fp16."""
+    name = _f16("vj_cross_attn_bwd", q)
     for t, n in ((q, "q"), (kv, "kv"), (out, "out"), (dout, "dout"), (dkv, "dkv")):
-        _chk(t, BF16, n)
+        _chk(t, q.dtype, n)
     _chk(lse2, F32, "lse2"); _chk(dq, F32, "dq")
     need = _lib.load().vj_cross_attn_bwd_workspace(B, nq, S, H, hd)
     ws = torch.empty(max(need, 4), dtype=torch.uint8, device=q.device)
-    _lib.call("vj_cross_attn_bwd", _p(q), _p(kv), _p(out), _p(dout), _p(lse2), _p(dq), _p(dkv), _p(ws), ws.numel(),
+    _lib.call(name, _p(q), _p(kv), _p(out), _p(dout), _p(lse2), _p(dq), _p(dkv), _p(ws), ws.numel(),
               B, nq, S, H, hd, float(scale), _s())
     return dq, dkv
 

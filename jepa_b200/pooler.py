@@ -14,6 +14,15 @@ FlatGradScaler and step.clip_grad_norm_ each take one launch over it.  Several p
 segment without attend_across_segments) accumulate into the same buffer.  `proj` gets no gradient: the reference builds
 it but never applies it (modules.py:152-153).  Gradients into the encoder's tokens (fine-tuning) and depth > 1 are not
 implemented.
+
+Precision: the probe computes bf16 x bf16 -> fp32 by default, inside an autocast region or not.  Built with
+`follow_autocast=True`, it follows an fp16 autocast (torch.autocast('cuda', dtype=torch.float16) or
+torch.cuda.amp.autocast(dtype=torch.float16), as the reference's eval loops open, eval.py:323): every 16-bit operand and
+activation is then fp16 (the fp16 shadow of the store, vj_gemm_f16, vj_cross_attn_*_f16, vj_layernorm_bwd_f16,
+vj_colsum_f16), while the residual stream, the LayerNorm statistics, lse2, dq and every weight gradient stay fp32.  The
+outputs then have the dtypes the reference's modules return under that autocast: fp16 logits from AttentiveClassifier,
+fp32 from AttentivePooler(complete_block=True), fp16 from AttentivePooler(complete_block=False).  Outside autocast, or
+under a bf16 autocast, such a probe computes in bf16 as by default.
 """
 import math
 from types import SimpleNamespace
@@ -27,7 +36,7 @@ from .params import FlatParamStore
 from .pos_embs import get_1d_sincos_pos_embed
 from .tensors import apply_masks, trunc_normal_
 
-BF16, F32 = torch.bfloat16, torch.float32
+BF16, F16, F32 = torch.bfloat16, torch.float16, torch.float32
 
 
 def _pad_rows(n, mult):
@@ -87,8 +96,9 @@ class AttentivePooler(nn.Module):
     """attentive_pooler.py:21-102."""
 
     def __init__(self, num_queries=1, embed_dim=768, num_heads=12, mlp_ratio=4.0, depth=1, norm_layer=nn.LayerNorm,
-                 init_std=0.02, qkv_bias=True, complete_block=True):
+                 init_std=0.02, qkv_bias=True, complete_block=True, follow_autocast=False):
         super().__init__()
+        self.follow_autocast = follow_autocast       # a plain attribute: not a parameter, not in the state_dict
         if depth != 1:
             raise NotImplementedError("AttentivePooler depth > 1 (extra self-attention blocks over the query tokens) is not "
                                       "used by the frozen evaluations (eval.py:182-187 builds depth=1)")
@@ -133,7 +143,8 @@ class AttentivePooler(nn.Module):
         _invalidate(self)
 
     def forward(self, x):
-        """x [B, S, D] encoder tokens -> pooled query tokens fp32 [B, num_queries, D]."""
+        """x [B, S, D] encoder tokens -> pooled query tokens [B, num_queries, D], fp32 (fp16 with complete_block=False
+        under an fp16 autocast that the probe follows)."""
         return _run_probe(self, self, x, head=False)
 
 
@@ -165,12 +176,14 @@ def _run_probe(module, pooler, x, head):
         raise NotImplementedError("the accelerated attentive probe trains the probe only: gradients into the encoder's "
                                   "tokens (fine-tuning) are not implemented - pass detached tokens")
     store, prefix = _store_of(module, pooler.query_tokens)
-    store.refresh_shadow()
+    dt = K.compute_dtype() if getattr(module, "follow_autocast", False) else BF16
+    store.refresh_shadow(dt)
     if not train:
         with torch.no_grad():
-            y, _ = _probe_forward(pooler, store, prefix, x, head, save=False)
+            y, _ = _probe_forward(pooler, store, prefix, x, head, save=False, dt=dt)
         return y
-    return _ProbeFn.apply(pooler, store, prefix, x, head, getattr(module, "_vj_probe_sync", None), *module.parameters())
+    return _ProbeFn.apply(pooler, store, prefix, x, head, dt, getattr(module, "_vj_probe_sync", None),
+                          *module.parameters())
 
 
 class _ProbeFn(torch.autograd.Function):
@@ -180,8 +193,8 @@ class _ProbeFn(torch.autograd.Function):
     the parameters.  proj is left without a gradient, as in the reference."""
 
     @staticmethod
-    def forward(ctx, pooler, store, prefix, x, head, sync, *params):
-        y, sv = _probe_forward(pooler, store, prefix, x, head, save=True)
+    def forward(ctx, pooler, store, prefix, x, head, dt, sync, *params):
+        y, sv = _probe_forward(pooler, store, prefix, x, head, save=True, dt=dt)
         ctx.pooler, ctx.store, ctx.prefix, ctx.sv, ctx.head, ctx.params = pooler, store, prefix, sv, head, params
         ctx.sync = sync
         return y
@@ -197,7 +210,7 @@ class _ProbeFn(torch.autograd.Function):
                 ctx.sync.mark(gflat)
         n = len(ctx.params)
         ctx.sv = ctx.params = ctx.sync = None
-        return (None, None, None, None, None, None) + (None,) * n
+        return (None,) * 7 + (None,) * n
 
 
 def _names(pooler, prefix):
@@ -205,39 +218,43 @@ def _names(pooler, prefix):
     return blk, (blk + "xattn." if pooler.complete_block else blk)
 
 
-def _probe_forward(pooler, store, prefix, x, head, save):
-    """Pooler (+ linear head) forward.  Returns (pooled fp32 [B, nq, D] or logits fp32 [B, C], saved activations)."""
+def _probe_forward(pooler, store, prefix, x, head, save, dt=BF16):
+    """Pooler (+ linear head) forward with 16-bit operands of dtype dt (bf16, or fp16 under an fp16 autocast the probe
+    follows).  Returns (pooled [B, nq, D] or logits [B, C], saved activations): fp32, except the fp16 logits and the fp16
+    pooled tokens of complete_block=False when dt is fp16."""
     B, S, D = x.shape
     H, nq, dev = pooler.num_heads, pooler.num_queries, x.device
     hd = D // H
     blk, xa = _names(pooler, prefix)
-    w = store.bf16
+    w = lambda name: store.w16(name, dt)
     f = store.f32
     has_qkv_bias = (xa + "kv.bias") in store.offsets
     x2 = x.detach().reshape(B * S, D).contiguous()
-    if x2.dtype not in (BF16, F32):
+    # fp16 LayerNorm reads fp16 or fp32 only (under autocast the encoder hands fp32); training in fp16 reads fp16 tokens
+    # as fp32 (exact), because the LayerNorm backward pairs its fp16 dy with an fp32 x
+    if x2.dtype not in (dt, F32) or (dt == F16 and save and x2.dtype == F16):
         x2 = x2.float()
-    sv = SimpleNamespace(B=B, S=S, x2=x2) if save else None
+    sv = SimpleNamespace(B=B, S=S, x2=x2, dt=dt) if save else None
     # keys / values: kv(norm1(x)) - one LayerNorm pass and one [B*S, 2D] GEMM (bias in the epilogue)
     if pooler.complete_block:
-        xn = torch.empty(B * S, D, dtype=BF16, device=dev)
+        xn = torch.empty(B * S, D, dtype=dt, device=dev)
         mean1 = torch.empty(B * S, dtype=F32, device=dev) if save else None
         rstd1 = torch.empty(B * S, dtype=F32, device=dev) if save else None
         K.layernorm_fwd(x2, xn, f(blk + "norm1.weight"), f(blk + "norm1.bias"), pooler.cross_attention_block.norm1.eps,
                         mean1, rstd1)
     else:
-        xn = x2 if x2.dtype == BF16 else x2.to(BF16)
+        xn = x2 if x2.dtype == dt else x2.to(dt)
         mean1 = rstd1 = None
-    kv = torch.empty(B * S, 2 * D, dtype=BF16, device=dev)
+    kv = torch.empty(B * S, 2 * D, dtype=dt, device=dev)
     K.gemm(xn, w(xa + "kv.weight"), kv, bias=f(xa + "kv.bias") if has_qkv_bias else None)
     # queries: the learned tokens, identical for every clip -> project once, repeat (rows padded to 8 for 16-byte rows)
     q0 = f(prefix + "query_tokens").reshape(nq, D)
-    q0b = torch.zeros(_pad_rows(nq, 8), D, dtype=BF16, device=dev)
-    q0b[:nq] = q0.to(BF16)
-    qp = torch.empty(_pad_rows(nq, 8), D, dtype=BF16, device=dev)
+    q0b = torch.zeros(_pad_rows(nq, 8), D, dtype=dt, device=dev)
+    q0b[:nq] = q0.to(dt)
+    qp = torch.empty(_pad_rows(nq, 8), D, dtype=dt, device=dev)
     K.gemm(q0b, w(xa + "q.weight"), qp, bias=f(xa + "q.bias") if has_qkv_bias else None)
     qrep = qp[:nq].repeat(B, 1).contiguous()                       # [B*nq, D], row b*nq + j = query j of clip b
-    att = torch.empty(B * nq, D, dtype=BF16, device=dev)
+    att = torch.empty(B * nq, D, dtype=dt, device=dev)
     if save:
         lse2 = torch.empty(B * nq, H, dtype=F32, device=dev)
         K.cross_attn_fwd_lse(qrep, kv, att, lse2, B, nq, S, H, hd, pooler.cross_attention_block.xattn.scale
@@ -248,20 +265,20 @@ def _probe_forward(pooler, store, prefix, x, head, save):
                          if pooler.complete_block else pooler.cross_attention_block.scale)
     M = _pad_rows(B * nq, 8)
     if not pooler.complete_block:
-        pooled = att.float()
+        pooled = att.clone() if dt == F16 else att.float()     # SDPA's output dtype under fp16 autocast (att is saved)
     else:
         # q = q + y ; q = q + fc2(gelu(fc1(norm2(q))))   (fp32 residual stream: it is only B*nq rows)
         q1p = torch.zeros(M, D, dtype=F32, device=dev)
         q1p[:B * nq] = q0.repeat(B, 1) + att.float()
-        ln2 = torch.empty(M, D, dtype=BF16, device=dev)
+        ln2 = torch.empty(M, D, dtype=dt, device=dev)
         mean2 = torch.empty(M, dtype=F32, device=dev) if save else None
         rstd2 = torch.empty(M, dtype=F32, device=dev) if save else None
         K.layernorm_fwd(q1p, ln2, f(blk + "norm2.weight"), f(blk + "norm2.bias"), pooler.cross_attention_block.norm2.eps,
                         mean2, rstd2)
         hid = store.offsets[blk + "mlp.fc1.weight"][2][0]
-        g = torch.empty(M, hid, dtype=BF16, device=dev)
+        g = torch.empty(M, hid, dtype=dt, device=dev)
         # training keeps gelu'(pre-activation) from the same epilogue: the fc1 dgrad is then a plain multiply
-        h = torch.empty(M, hid, dtype=BF16, device=dev) if save else None
+        h = torch.empty(M, hid, dtype=dt, device=dev) if save else None
         K.gemm(ln2, w(blk + "mlp.fc1.weight"), g, bias=f(blk + "mlp.fc1.bias"), epi=K.EPI_GELU_GRAD if save else K.EPI_GELU,
                aux_out=h)
         q2 = torch.empty(M, D, dtype=F32, device=dev)
@@ -275,22 +292,24 @@ def _probe_forward(pooler, store, prefix, x, head, save):
     # straight from the store for any class count; the bias comes in through the residual epilogue
     C = store.offsets["linear.weight"][2][0]
     Np = _pad_rows(B, 64)
-    pb = torch.zeros(Np, D, dtype=BF16, device=dev)
+    pb = torch.zeros(Np, D, dtype=dt, device=dev)
     pb[:B] = pooled
     bias_t = f("linear.bias").unsqueeze(1).expand(C, Np).contiguous()
     lt = torch.empty(C, Np, dtype=F32, device=dev)
     K.gemm(w("linear.weight"), pb, lt, epi=K.EPI_ADD, aux=bias_t)
     if save:
         sv.pb = pb
-    return lt[:, :B].t().contiguous(), sv
+    logits = lt[:, :B].t()
+    # nn.Linear under fp16 autocast returns fp16: the fp32 accumulator plus bias, rounded once (past 65504: +-inf)
+    return (logits.to(F16) if dt == F16 else logits).contiguous(), sv
 
 
 def _probe_backward(pooler, store, prefix, sv, dy, head, gflat):
-    B, S, D = sv.B, sv.S, sv.x2.shape[1]
+    B, S, D, dt = sv.B, sv.S, sv.x2.shape[1], sv.dt
     H, nq, dev = pooler.num_heads, pooler.num_queries, gflat.device
     hd = D // H
     blk, xa = _names(pooler, prefix)
-    w = store.bf16
+    w = lambda name: store.w16(name, dt)
     f = store.f32
     gv = lambda name: store.grad_view(gflat, name)
     has_qkv_bias = (xa + "kv.bias") in store.offsets
@@ -300,7 +319,7 @@ def _probe_backward(pooler, store, prefix, sv, dy, head, gflat):
         C = store.offsets["linear.weight"][2][0]
         Np = sv.pb.shape[0]
         dl = dy.detach().to(F32)
-        dlt = torch.zeros(C, Np, dtype=BF16, device=dev)
+        dlt = torch.zeros(C, Np, dtype=dt, device=dev)
         dlt[:, :B] = dl.t()
         K.gemm(dlt, sv.pb, gv("linear.weight"), b_mn=True, accumulate=True)
         Cp = _pad_rows(C, 8)      # colsum works on 8-column groups: the bias slice is followed by store padding
@@ -317,13 +336,13 @@ def _probe_backward(pooler, store, prefix, sv, dy, head, gflat):
         dq2[:M] = dy.detach().reshape(M, D)
     if pooler.complete_block:
         # MLP: q2 = q1 + fc2(gelu(fc1(ln2(q1))))
-        dq2b = dq2.to(BF16)
+        dq2b = dq2.to(dt)
         _wgrad(dq2b, sv.g, gv(blk + "mlp.fc2.weight"), gv(blk + "mlp.fc2.bias"), Mp)
         hid = sv.g.shape[1]
-        dpre = torch.empty(Mp, hid, dtype=BF16, device=dev)
+        dpre = torch.empty(Mp, hid, dtype=dt, device=dev)
         K.gemm(dq2b, w(blk + "mlp.fc2.weight"), dpre, b_mn=True, epi=K.EPI_MUL, aux=sv.h)
         _wgrad(dpre, sv.ln2, gv(blk + "mlp.fc1.weight"), gv(blk + "mlp.fc1.bias"), Mp)
-        dln2 = torch.empty(Mp, D, dtype=BF16, device=dev)
+        dln2 = torch.empty(Mp, D, dtype=dt, device=dev)
         K.gemm(dpre, w(blk + "mlp.fc1.weight"), dln2, b_mn=True)
         dq1 = torch.empty(Mp, D, dtype=F32, device=dev)
         K.layernorm_bwd(dln2, sv.q1p, f(blk + "norm2.weight"), sv.mean2, sv.rstd2, dq2, dq1, gv(blk + "norm2.weight"),
@@ -331,9 +350,9 @@ def _probe_backward(pooler, store, prefix, sv, dy, head, gflat):
     else:
         dq1 = dq2
     # cross-attention
-    datt = dq1[:M].to(BF16)
+    datt = dq1[:M].to(dt)
     dqrep = torch.empty(M, D, dtype=F32, device=dev)
-    dkv = torch.empty(B * S, 2 * D, dtype=BF16, device=dev)
+    dkv = torch.empty(B * S, 2 * D, dtype=dt, device=dev)
     scale = pooler.cross_attention_block.xattn.scale if pooler.complete_block else pooler.cross_attention_block.scale
     K.cross_attn_bwd(sv.qrep, sv.kv, sv.att, datt, sv.lse2, dqrep, dkv, B, nq, S, H, hd, scale)
     # the query projection is shared by all clips: sum its gradient over them (row b*nq + j -> query j)
@@ -343,7 +362,7 @@ def _probe_backward(pooler, store, prefix, sv, dy, head, gflat):
         K.colsum(dqrep, dqp[j], period=nq, lo=j, hi=j + 1)
         if pooler.complete_block:      # residual path q1 = q0 + y
             K.colsum(dq1[:M], gq[j], period=nq, lo=j, hi=j + 1)
-    dqpb = dqp.to(BF16)
+    dqpb = dqp.to(dt)
     _wgrad(dqpb, sv.q0b, gv(xa + "q.weight"), None, dqpb.shape[0])
     if has_qkv_bias:
         K.colsum(dqp, gv(xa + "q.bias"))
@@ -352,7 +371,7 @@ def _probe_backward(pooler, store, prefix, sv, dy, head, gflat):
     _wgrad(dkv, sv.xn, gv(xa + "kv.weight"), gv(xa + "kv.bias") if has_qkv_bias else None, B * S)
     if pooler.complete_block:
         # norm1's affine parameters only: the gradient into the frozen encoder's tokens goes to scratch
-        dxn = torch.empty(B * S, D, dtype=BF16, device=dev)
+        dxn = torch.empty(B * S, D, dtype=dt, device=dev)
         K.gemm(dkv, w(xa + "kv.weight"), dxn, b_mn=True)
         dx = torch.empty_like(sv.x2)
         K.layernorm_bwd(dxn, sv.x2, f(blk + "norm1.weight"), sv.mean1, sv.rstd1, None, dx, gv(blk + "norm1.weight"),
@@ -372,11 +391,12 @@ class AttentiveClassifier(nn.Module):
     """attentive_pooler.py:105-136: pooler (one query token) + linear head."""
 
     def __init__(self, embed_dim=768, num_heads=12, mlp_ratio=4.0, depth=1, norm_layer=nn.LayerNorm, init_std=0.02,
-                 qkv_bias=True, num_classes=1000, complete_block=True):
+                 qkv_bias=True, num_classes=1000, complete_block=True, follow_autocast=False):
         super().__init__()
+        self.follow_autocast = follow_autocast       # a plain attribute: not a parameter, not in the state_dict
         self.pooler = AttentivePooler(num_queries=1, embed_dim=embed_dim, num_heads=num_heads, mlp_ratio=mlp_ratio,
                                       depth=depth, norm_layer=norm_layer, init_std=init_std, qkv_bias=qkv_bias,
-                                      complete_block=complete_block)
+                                      complete_block=complete_block, follow_autocast=follow_autocast)
         self.linear = nn.Linear(embed_dim, num_classes, bias=True)
         self._store = FlatParamStore()
 
@@ -385,7 +405,8 @@ class AttentiveClassifier(nn.Module):
         _invalidate(self)
 
     def forward(self, x):
-        """x [B, S, D] encoder tokens -> logits fp32 [B, num_classes]."""
+        """x [B, S, D] encoder tokens -> logits [B, num_classes]: fp32, or fp16 under an fp16 autocast the classifier
+        follows."""
         return _run_probe(self, self.pooler, x, head=True)
 
 

@@ -1,7 +1,16 @@
 #!/usr/bin/env python
 """Frozen-evaluation probe training step (or validation step), clips/sec, at the ViT-L/16 K400 shape.
 
-    python tools/bench_probe.py [--steps K] [--warmup W] [--batch B] [--mode train|val|image]
+    python tools/bench_probe.py [--steps K] [--warmup W] [--batch B] [--mode train|val|image|xattn]
+                                [--dtype bfloat16|float16]
+
+--dtype float16 runs each step's encoder and classifier calls inside the reference's autocast(dtype=torch.float16)
+region (evals/video_classification_frozen/eval.py:323) with AttentiveClassifier(follow_autocast=True): fp16 encoder,
+fp16 probe forward and backward, fp16 logits, GradScaler.  The default bfloat16 is the evaluation loop without autocast.
+
+--mode xattn times vj_cross_attn_fwd_lse and vj_cross_attn_bwd alone, bf16 and fp16 alternating, at the K400 probe
+shapes (B 4, S 12 544, one query; ViT-L H 16 x hd 64 and ViT-H H 16 x hd 80), and reports GB/s from the bytes each must
+move (the kv read, the dkv write).
 
 --uint8 (train mode) starts each step from B x 8 uint8 clips [16, 256, 340, 3] on the host: the evaluation's training
 transform draws its decisions there (RandAugment, crop, erase), then augment_batch runs them on the GPU; it reports the
@@ -30,6 +39,7 @@ encoder-forward and probe fwd + bwd + optimiser times (CUDA events), the card's 
 nvidia-smi sampled during the timed steps.  Writes nothing into the repository.
 """
 import argparse
+import contextlib
 import json
 import os
 import subprocess
@@ -45,6 +55,13 @@ import torch  # noqa: E402
 from bench import ClockSampler  # noqa: E402
 
 
+def _region(args):
+    """The reference's loop-body autocast region with --dtype float16, none with bfloat16."""
+    if args.dtype == "float16":
+        return torch.autocast("cuda", dtype=torch.float16)
+    return contextlib.nullcontext()
+
+
 def run(args):
     from jepa_b200.models import vit_large
     from jepa_b200.optim import FlatAdamW, FlatGradScaler
@@ -56,7 +73,8 @@ def run(args):
     n_seg, frames, crop, n_cls = 8, 16, 224, 400
     enc = vit_large(img_size=crop, num_frames=frames, tubelet_size=2, uniform_power=True).to(device).eval()
     encoder = ClipAggregation(enc, tubelet_size=2, attend_across_segments=True)
-    clf = AttentiveClassifier(embed_dim=enc.embed_dim, num_heads=enc.num_heads, depth=1, num_classes=n_cls).to(device)
+    clf = AttentiveClassifier(embed_dim=enc.embed_dim, num_heads=enc.num_heads, depth=1, num_classes=n_cls,
+                              follow_autocast=args.dtype == "float16").to(device)
     groups = [{"params": [p for n, p in clf.named_parameters() if ("bias" not in n) and (len(p.shape) != 1)]},
               {"params": [p for n, p in clf.named_parameters() if ("bias" in n) or (len(p.shape) == 1)],
                "WD_exclude": True, "weight_decay": 0}]
@@ -90,11 +108,13 @@ def run(args):
                 aug_bytes.append(_augment_bytes(tickets, pack_augment, out))
         if timed:
             ev[0].record()
-        with torch.no_grad():
-            outputs = encoder(clips)
-        if timed:
-            ev[1].record()
-        loss = sum([crit(clf(o), labels) for o in outputs]) / len(outputs)
+        with _region(args):
+            with torch.no_grad():
+                outputs = encoder(clips)
+            if timed:
+                ev[1].record()
+            logits = [clf(o) for o in outputs]
+        loss = sum([crit(o, labels) for o in logits]) / len(logits)
         scaler.scale(loss).backward()
         scaler.unscale_(opt)
         clip_grad_norm_(clf, 1.0)
@@ -138,7 +158,7 @@ def run(args):
     print(json.dumps({
         "metric": "clips/sec ViT-L/16 K400 frozen-evaluation probe training step (8x16x224^2 per clip, 400 classes)",
         "value": round(B * args.steps / wall, 2), "unit": "clips/s", "n_gpus": 1, "steps": args.steps,
-        "warmup": args.warmup, "higher_is_better": True, "dtype": "bf16", "data": "synthetic",
+        "warmup": args.warmup, "higher_is_better": True, "dtype": args.dtype, "data": "synthetic",
         "config": {"workload": f"batch {B}/GPU, {n_seg} segments x {frames} frames, attend_across_segments "
                                f"({n_seg * enc.num_patches} tokens per clip), AttentiveClassifier depth 1, "
                                "CrossEntropyLoss, FlatGradScaler + clip 1.0 + FlatAdamW"},
@@ -210,7 +230,8 @@ def run_val(args):
     for p in enc.parameters():          # frozen, as in the evaluation: the forward keeps no activations
         p.requires_grad = False
     encoder = ClipAggregation(enc, tubelet_size=2, attend_across_segments=True)
-    clf = AttentiveClassifier(embed_dim=enc.embed_dim, num_heads=enc.num_heads, depth=1, num_classes=n_cls).to(device).eval()
+    clf = AttentiveClassifier(embed_dim=enc.embed_dim, num_heads=enc.num_heads, depth=1, num_classes=n_cls,
+                              follow_autocast=args.dtype == "float16").to(device).eval()
     g = torch.Generator().manual_seed(0)
     segments = [torch.randint(0, 256, (B, frames, H0, W0, 3), dtype=torch.uint8, generator=g).pin_memory()
                 for _ in range(n_seg)]
@@ -224,7 +245,8 @@ def run_val(args):
             clips = preprocess_views(segments, device, crop, n_views)
             if timed:
                 ev[1].record()
-            outputs = [clf(o) for o in encoder(clips)]
+            with _region(args):
+                outputs = [clf(o) for o in encoder(clips)]
             probs = sum([F.softmax(o, dim=1) for o in outputs]) / len(outputs)
         if timed:
             ev[2].record()
@@ -267,7 +289,7 @@ def run_val(args):
         "metric": "clips/sec ViT-L/16 K400 frozen-evaluation validation step (8 segments x 3 views x 16x224^2 per clip, "
                   "uint8 frames in)",
         "value": round(B * args.steps / wall, 2), "unit": "clips/s", "n_gpus": 1, "steps": args.steps,
-        "warmup": args.warmup, "higher_is_better": True, "dtype": "bf16", "data": "synthetic uint8",
+        "warmup": args.warmup, "higher_is_better": True, "dtype": args.dtype, "data": "synthetic uint8",
         "config": {"workload": f"batch {B}/GPU, {n_seg} segments x {n_views} views of {frames} frames from uint8 "
                                f"{H0}x{W0} frames (EvalVideoTransform via vj_clip_views), attend_across_segments, "
                                f"{n_views} classifier calls, softmax average"},
@@ -298,7 +320,8 @@ def run_image(args):
     enc = vit_large(img_size=crop, num_frames=frames, tubelet_size=2, uniform_power=True).to(device).eval()
     for p in enc.parameters():
         p.requires_grad = False
-    clf = AttentiveClassifier(embed_dim=enc.embed_dim, num_heads=enc.num_heads, depth=1, num_classes=n_cls).to(device)
+    clf = AttentiveClassifier(embed_dim=enc.embed_dim, num_heads=enc.num_heads, depth=1, num_classes=n_cls,
+                              follow_autocast=args.dtype == "float16").to(device)
     groups = [{"params": [p for n, p in clf.named_parameters() if ("bias" not in n) and (len(p.shape) != 1)]},
               {"params": [p for n, p in clf.named_parameters() if ("bias" in n) or (len(p.shape) == 1)],
                "WD_exclude": True, "weight_decay": 0}]
@@ -324,11 +347,13 @@ def run_image(args):
             imgs = tf.batch(tickets, device)
         if timed:
             ev[0].record()
-        with torch.no_grad():
-            outputs = enc(imgs.unsqueeze(2).repeat(1, 1, frames, 1, 1))
-        if timed:
-            ev[1].record()
-        loss = crit(clf(outputs), labels)
+        with _region(args):
+            with torch.no_grad():
+                outputs = enc(imgs.unsqueeze(2).repeat(1, 1, frames, 1, 1))
+            if timed:
+                ev[1].record()
+            logits = clf(outputs)
+        loss = crit(logits, labels)
         scaler.scale(loss).backward()
         scaler.unscale_(opt)
         clip_grad_norm_(clf, 1.0)
@@ -381,7 +406,7 @@ def run_image(args):
     print(json.dumps({
         "metric": "images/sec ViT-L/16 in1k frozen-evaluation probe training step (16x224^2 per image, 1000 classes)",
         "value": round(B * args.steps / wall, 2), "unit": "images/s", "n_gpus": 1, "steps": args.steps,
-        "warmup": args.warmup, "higher_is_better": True, "dtype": "bf16",
+        "warmup": args.warmup, "higher_is_better": True, "dtype": args.dtype,
         "data": (f"uint8 {W0}x{H0} images on the host, timm AutoAugment 'original' + erasing 0.25 on the GPU"
                  if args.uint8 else "pre-normalised images resident on the device"),
         "config": {"workload": f"batch {B}/GPU, each image repeated over {frames} frames ({enc.num_patches} tokens), "
@@ -440,19 +465,78 @@ def _reference_image_cpu_ms(img, crop):
         return None
 
 
+def run_xattn(args):
+    """vj_cross_attn_fwd_lse / vj_cross_attn_bwd (+ its dq reduce) alone, bf16 and fp16 alternating per repetition."""
+    from jepa_b200 import kernels as K
+    device = torch.device("cuda:0")
+    B, S, H, nq = args.batch or 4, 12544, 16, 1
+    g = torch.Generator(device="cpu").manual_seed(0)
+    ev = [torch.cuda.Event(enable_timing=True) for _ in range(3)]
+    rows = []
+    for hd in (64, 80):
+        D = H * hd
+        ref = {"q": torch.randn(B * nq, D, generator=g), "kv": torch.randn(B * S, 2 * D, generator=g),
+               "dout": torch.randn(B * nq, D, generator=g)}
+        bufs = {}
+        for dt in (torch.bfloat16, torch.float16):
+            t = {k: v.to(device, dt) for k, v in ref.items()}
+            t["out"] = torch.empty(B * nq, D, dtype=dt, device=device)
+            t["dkv"] = torch.empty(B * S, 2 * D, dtype=dt, device=device)
+            t["lse"] = torch.empty(B * nq, H, device=device)
+            t["dq"] = torch.empty(B * nq, D, device=device)
+            bufs[dt] = t
+        times = {dt: ([], []) for dt in bufs}
+        for i in range(args.warmup + args.steps):
+            for dt, t in bufs.items():
+                ev[0].record()
+                K.cross_attn_fwd_lse(t["q"], t["kv"], t["out"], t["lse"], B, nq, S, H, hd, hd ** -0.5)
+                ev[1].record()
+                K.cross_attn_bwd(t["q"], t["kv"], t["out"], t["dout"], t["lse"], t["dq"], t["dkv"], B, nq, S, H, hd,
+                                 hd ** -0.5)
+                ev[2].record()
+                torch.cuda.synchronize()
+                if i >= args.warmup:
+                    times[dt][0].append(ev[0].elapsed_time(ev[1]))
+                    times[dt][1].append(ev[1].elapsed_time(ev[2]))
+        kv_bytes = B * S * 2 * D * 2
+        for dt, (f, b) in times.items():
+            fm, bm = sorted(f)[len(f) // 2], sorted(b)[len(b) // 2]
+            rows.append({"hd": hd, "dtype": str(dt).replace("torch.", ""), "fwd_ms": round(fm, 4),
+                         "bwd_ms": round(bm, 4), "fwd_gbps": round(kv_bytes / (fm * 1e-3) / 1e9, 1),
+                         "bwd_gbps": round(2 * kv_bytes / (bm * 1e-3) / 1e9, 1),
+                         "fwd_ms_min_max": [round(min(f), 4), round(max(f), 4)],
+                         "bwd_ms_min_max": [round(min(b), 4), round(max(b), 4)]})
+    card = _card()
+    print(json.dumps({
+        "metric": "cross-attention forward (with lse) and backward, bf16 vs fp16, K400 probe shape",
+        "config": {"workload": f"B {B}, S {S}, H {H}, nq {nq}, hd 64 (ViT-L) and 80 (ViT-H)"},
+        "rows": rows,
+        "timing": "CUDA events around each launch (backward: both kernels), median over the timed repetitions, the two "
+                  "dtypes alternating; GB/s from the kv read (forward) and the kv read + dkv write (backward)",
+        "gpu": card[0] if card else None,
+        "power_limit_w": float(card[1]) if len(card) > 1 else None,
+    }), flush=True)
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--steps", type=int, default=10)
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--batch", type=int, default=None,
                     help="clips (images) per step; default 4 (K400 eval config) or, in image mode, 16 (in1k config)")
-    ap.add_argument("--mode", choices=("train", "val", "image"), default="train",
-                    help="train: probe training step; val: validation step from uint8 frames; image: image probe step")
+    ap.add_argument("--mode", choices=("train", "val", "image", "xattn"), default="train",
+                    help="train: probe training step; val: validation step from uint8 frames; image: image probe step; "
+                         "xattn: the cross-attention kernels alone, bf16 against fp16")
+    ap.add_argument("--dtype", choices=("bfloat16", "float16"), default="bfloat16",
+                    help="float16: encoder and probe under the reference's autocast(float16) region")
     ap.add_argument("--uint8", action="store_true",
                     help="train / image mode: uint8 frames / images through the GPU training transform")
     args = ap.parse_args()
     if args.mode == "image":
         run_image(args)
+        return
+    if args.mode == "xattn":
+        run_xattn(args)
         return
     args.batch = args.batch or 4
     run(args) if args.mode == "train" else run_val(args)
