@@ -10,6 +10,9 @@ By default this loop opens no autocast region, so encoder and probe compute bf16
 selects the GradScaler, as it does in the reference.  `optimization.fp16_autocast: true` opens that region where the
 reference does and builds the classifier to follow it, exactly as in the video evaluation: fp16 encoder and probe with
 `use_bfloat16: true`, bf16 throughout with `use_bfloat16: false`.  There is no fp32 path.
+
+`optimization.multihead_kwargs` trains several probes on one encoder pass per batch, with the video evaluation's parser,
+head construction, epoch loop, checkpoint and CSV layout (read_multihead_kwargs, build_heads, train_heads).
 """
 import os
 
@@ -27,8 +30,9 @@ import torch
 import torch.multiprocessing as mp
 
 import src.models.vision_transformer as vit
-from evals.video_classification_frozen.eval import (init_opt, load_checkpoint, load_pretrained, loop_autocast,
-                                                    read_fp16_autocast, require_cuda)
+from evals.video_classification_frozen.eval import (build_heads, init_opt, load_checkpoint, load_pretrained,
+                                                    loop_autocast, read_fp16_autocast, read_multihead_kwargs,
+                                                    require_cuda, step_head, train_heads)
 from src.datasets.data_manager import init_data
 from src.models.attentive_pooler import AttentiveClassifier
 from src.utils.distributed import AllReduce, DistributedDataParallel, init_distributed
@@ -80,6 +84,7 @@ def main(args_eval, resume_preempt=False):
     warmup = args_opt.get('warmup')
     use_bfloat16 = args_opt.get('use_bfloat16')
     fp16_autocast = read_fp16_autocast(args_opt)
+    multihead_kwargs = read_multihead_kwargs(args_opt)
 
     resume_checkpoint = args_eval.get('resume_checkpoint', False) or resume_preempt
     eval_tag = args_eval.get('tag', None)
@@ -102,7 +107,7 @@ def main(args_eval, resume_preempt=False):
     log_file = os.path.join(folder, f'{tag}_r{rank}.csv')
     latest_path = os.path.join(folder, f'{tag}-latest.pth.tar')
 
-    if rank == 0:
+    if rank == 0 and multihead_kwargs is None:
         csv_logger = CSVLogger(log_file, ('%d', 'epoch'), ('%.5f', 'loss'), ('%.5f', 'acc'))
 
     encoder = init_model(crop_size=resolution, device=device, pretrained=pretrained_path, model_name=model_name,
@@ -113,8 +118,10 @@ def main(args_eval, resume_preempt=False):
     for p in encoder.parameters():
         p.requires_grad = False
 
-    classifier = AttentiveClassifier(embed_dim=encoder.embed_dim, num_heads=encoder.num_heads, depth=1,
-                                     num_classes=num_classes, follow_autocast=fp16_autocast).to(device)
+    classifiers = build_heads(lambda: AttentiveClassifier(embed_dim=encoder.embed_dim, num_heads=encoder.num_heads,
+                                                          depth=1, num_classes=num_classes,
+                                                          follow_autocast=fp16_autocast).to(device),
+                              1 if multihead_kwargs is None else len(multihead_kwargs))
 
     train_loader = make_dataloader(dataset_name=dataset_name, root_path=root_path, resolution=resolution,
                                    image_folder=image_folder, batch_size=batch_size, world_size=world_size, rank=rank,
@@ -125,6 +132,17 @@ def main(args_eval, resume_preempt=False):
     ipe = len(train_loader)
     logger.info(f'Dataloader created... iterations per epoch: {ipe}')
 
+    if multihead_kwargs is not None:
+        def run_epoch(training, heads):
+            return run_one_epoch(device=device, training=training, encoder=encoder,
+                                 data_loader=train_loader if training else val_loader, use_bfloat16=use_bfloat16,
+                                 fp16_autocast=fp16_autocast, **heads)
+        train_heads(classifiers, multihead_kwargs, run_epoch, iterations_per_epoch=ipe, num_epochs=num_epochs,
+                    use_bfloat16=use_bfloat16, resume_checkpoint=resume_checkpoint, latest_path=latest_path,
+                    log_file=log_file, device=device, rank=rank, world_size=world_size, batch_size=batch_size)
+        return
+
+    classifier = classifiers[0]
     optimizer, scaler, scheduler, wd_scheduler = init_opt(
         classifier=classifier, wd=wd, start_lr=start_lr, ref_lr=lr, final_lr=final_lr, iterations_per_epoch=ipe,
         warmup=warmup, num_epochs=num_epochs, use_bfloat16=use_bfloat16)
@@ -167,15 +185,21 @@ def main(args_eval, resume_preempt=False):
 
 def run_one_epoch(device, training, encoder, classifier, scaler, optimizer, scheduler, wd_scheduler, data_loader,
                   use_bfloat16, fp16_autocast=False):
-    """eval.py:262-317: one classifier call per step."""
-    classifier.train(mode=training)
+    """eval.py:262-317: one classifier call per step.  classifier, scaler, optimizer, scheduler and wd_scheduler may be
+    lists, one entry per head, as in the video evaluation's run_one_epoch: one encoder pass per batch, then each head's
+    loop body in turn; the per-head accuracies are returned."""
+    multi = isinstance(classifier, (list, tuple))
+    heads = list(zip(*[x if multi else [x] for x in (classifier, scaler, optimizer, scheduler, wd_scheduler)]))
+    for clf, *_ in heads:
+        clf.train(mode=training)
     criterion = torch.nn.CrossEntropyLoss()
-    top1_meter = AverageMeter()
+    top1_meters = [AverageMeter() for _ in heads]
     for itr, data in enumerate(data_loader):
 
         if training:
-            scheduler.step()
-            wd_scheduler.step()
+            for *_, sched, wd_sched in heads:
+                sched.step()
+                wd_sched.step()
 
         # (without fp16_autocast no region: encoder and probe compute bf16 x bf16 -> fp32; see the module docstring)
         with loop_autocast(fp16_autocast, use_bfloat16):
@@ -185,35 +209,28 @@ def run_one_epoch(device, training, encoder, classifier, scaler, optimizer, sche
                 imgs = data[0].to(device)
             labels = data[1].to(device)
             with torch.no_grad():
-                outputs = encoder(imgs)
-                if not training:
-                    outputs = classifier(outputs)
+                tokens = encoder(imgs)
+
+        for k, (clf, scaler, optimizer, _, _) in enumerate(heads):
+            # the classifier call runs in the same region as the encoder; validation under no_grad
+            with loop_autocast(fp16_autocast, use_bfloat16), torch.set_grad_enabled(training):
+                outputs = clf(tokens)
+
+            loss = criterion(outputs, labels)
+            top1_acc = 100. * outputs.max(dim=1).indices.eq(labels).sum() / len(imgs)
+            top1_acc = float(AllReduce.apply(top1_acc))
+            top1_meters[k].update(top1_acc)
+
             if training:
-                outputs = classifier(outputs)
+                step_head(clf, scaler, optimizer, loss, use_bfloat16)
 
-        loss = criterion(outputs, labels)
-        top1_acc = 100. * outputs.max(dim=1).indices.eq(labels).sum() / len(imgs)
-        top1_acc = float(AllReduce.apply(top1_acc))
-        top1_meter.update(top1_acc)
+            if itr % 20 == 0:
+                logger.info(('[%5d] head %d: ' % (itr, k) if multi else '[%5d] ' % itr)
+                            + '%.3f%% (loss: %.3f) [mem: %.2e]'
+                            % (top1_meters[k].avg, loss, torch.cuda.max_memory_allocated() / 1024.**2))
 
-        if training:
-            if use_bfloat16:
-                scaler.scale(loss).backward()
-                scaler.unscale_(optimizer)
-                torch.nn.utils.clip_grad_norm_(classifier.parameters(), 1.0)
-                scaler.step(optimizer)
-                scaler.update()
-            else:
-                loss.backward()
-                torch.nn.utils.clip_grad_norm_(classifier.parameters(), 1.0)
-                optimizer.step()
-            optimizer.zero_grad()
-
-        if itr % 20 == 0:
-            logger.info('[%5d] %.3f%% (loss: %.3f) [mem: %.2e]'
-                        % (itr, top1_meter.avg, loss, torch.cuda.max_memory_allocated() / 1024.**2))
-
-    return top1_meter.avg
+    accs = [m.avg for m in top1_meters]
+    return accs if multi else accs[0]
 
 
 def make_dataloader(dataset_name, root_path, image_folder, batch_size, world_size, rank, resolution=224, training=False,

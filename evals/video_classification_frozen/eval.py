@@ -16,8 +16,15 @@ that same region, where the reference opens it, and the classifier follows it (A
 with `use_bfloat16: true` the encoder, the probe's forward and its backward compute in fp16 as the reference's do, with
 fp16 logits and GradScaler; with `use_bfloat16: false` the region is disabled, as in the reference, and everything
 computes in bf16 as by default.  There is no fp32 path.
+
+`optimization.multihead_kwargs` (a list of per-head lr / start_lr / final_lr / weight_decay / final_weight_decay /
+warmup, read by read_multihead_kwargs) trains several probes ("heads") on one encoder pass per batch: every head starts
+from the same weights and has its own optimizer, schedules, GradScaler and gradient exchange (train_heads).  Without the
+key the driver trains one classifier with the reference's checkpoint, CSV and log lines.
 """
+import collections.abc
 import contextlib
+import math
 import os
 
 try:
@@ -105,6 +112,7 @@ def main(args_eval, resume_preempt=False):
     warmup = args_opt.get('warmup')
     use_bfloat16 = args_opt.get('use_bfloat16')
     fp16_autocast = read_fp16_autocast(args_opt)
+    multihead_kwargs = read_multihead_kwargs(args_opt)
 
     resume_checkpoint = args_eval.get('resume_checkpoint', False) or resume_preempt
     eval_tag = args_eval.get('tag', None)
@@ -127,7 +135,7 @@ def main(args_eval, resume_preempt=False):
     log_file = os.path.join(folder, f'{tag}_r{rank}.csv')
     latest_path = os.path.join(folder, f'{tag}-latest.pth.tar')
 
-    if rank == 0:
+    if rank == 0 and multihead_kwargs is None:
         csv_logger = CSVLogger(log_file, ('%d', 'epoch'), ('%.5f', 'loss'), ('%.5f', 'acc'))
 
     # -- pretrained encoder (frozen)
@@ -149,8 +157,10 @@ def main(args_eval, resume_preempt=False):
     for p in encoder.parameters():
         p.requires_grad = False
 
-    classifier = AttentiveClassifier(embed_dim=encoder.embed_dim, num_heads=encoder.num_heads, depth=1,
-                                     num_classes=num_classes, follow_autocast=fp16_autocast).to(device)
+    classifiers = build_heads(lambda: AttentiveClassifier(embed_dim=encoder.embed_dim, num_heads=encoder.num_heads,
+                                                          depth=1, num_classes=num_classes,
+                                                          follow_autocast=fp16_autocast).to(device),
+                              1 if multihead_kwargs is None else len(multihead_kwargs))
 
     train_loader = make_dataloader(dataset_type=dataset_type, root_path=train_data_path, resolution=resolution,
                                    frames_per_clip=eval_frames_per_clip, frame_step=eval_frame_step,
@@ -168,6 +178,20 @@ def main(args_eval, resume_preempt=False):
     ipe = len(train_loader)
     logger.info(f'Dataloader created... iterations per epoch: {ipe}')
 
+    if multihead_kwargs is not None:
+        def run_epoch(training, heads):
+            return run_one_epoch(device=device, training=training,
+                                 num_temporal_views=eval_num_segments if (attend_across_segments or not training) else 1,
+                                 attend_across_segments=attend_across_segments,
+                                 num_spatial_views=1 if training else eval_num_views_per_segment, encoder=encoder,
+                                 data_loader=train_loader if training else val_loader, use_bfloat16=use_bfloat16,
+                                 fp16_autocast=fp16_autocast, **heads)
+        train_heads(classifiers, multihead_kwargs, run_epoch, iterations_per_epoch=ipe, num_epochs=num_epochs,
+                    use_bfloat16=use_bfloat16, resume_checkpoint=resume_checkpoint, latest_path=latest_path,
+                    log_file=log_file, device=device, rank=rank, world_size=world_size, batch_size=batch_size)
+        return
+
+    classifier = classifiers[0]
     optimizer, scaler, scheduler, wd_scheduler = init_opt(
         classifier=classifier, wd=wd, start_lr=start_lr, ref_lr=lr, final_lr=final_lr, iterations_per_epoch=ipe,
         warmup=warmup, num_epochs=num_epochs, use_bfloat16=use_bfloat16)
@@ -230,6 +254,132 @@ def loop_autocast(fp16_autocast, use_bfloat16):
     return torch.autocast('cuda', dtype=torch.float16, enabled=bool(use_bfloat16))
 
 
+MULTIHEAD_FIELDS = ('lr', 'start_lr', 'final_lr', 'weight_decay', 'final_weight_decay', 'warmup')
+
+
+def read_multihead_kwargs(args_opt):
+    """`optimization.multihead_kwargs`: None when the key is absent (one classifier), else one resolved dict of
+    MULTIHEAD_FIELDS per head, as floats.  A field a head leaves out takes the top-level `optimization` value;
+    final_weight_decay defaults to 1e-6, the value init_opt uses for one classifier."""
+    if 'multihead_kwargs' not in args_opt:
+        return None
+    value = args_opt['multihead_kwargs']
+    if not isinstance(value, (list, tuple)) or len(value) == 0:
+        raise ValueError(f"optimization.multihead_kwargs must be a non-empty list of mappings, got {value!r}")
+    defaults = {'lr': args_opt.get('lr'), 'start_lr': args_opt.get('start_lr'), 'final_lr': args_opt.get('final_lr'),
+                'weight_decay': args_opt.get('weight_decay'), 'final_weight_decay': 1e-6, 'warmup': args_opt.get('warmup')}
+    heads = []
+    for i, entry in enumerate(value):
+        if not isinstance(entry, collections.abc.Mapping):
+            raise ValueError(f"optimization.multihead_kwargs[{i}] must be a mapping, got {entry!r}")
+        for key in entry:
+            if key not in MULTIHEAD_FIELDS:
+                raise ValueError(f"optimization.multihead_kwargs[{i}]: unknown key {key!r} "
+                                 f"(allowed: {', '.join(MULTIHEAD_FIELDS)})")
+        head = {}
+        for key in MULTIHEAD_FIELDS:
+            v = entry.get(key, defaults[key])
+            if isinstance(v, bool) or not isinstance(v, (int, float)) or not math.isfinite(v):
+                where = '' if key in entry else f' (from optimization.{key})'
+                raise ValueError(f"optimization.multihead_kwargs[{i}].{key} must be a finite number, got {v!r}{where}")
+            if v < 0:
+                raise ValueError(f"optimization.multihead_kwargs[{i}].{key} must not be negative, got {v!r}")
+            head[key] = float(v)
+        heads.append(head)
+    return heads
+
+
+def build_heads(make_classifier, num_heads):
+    """num_heads classifiers with equal initial weights.  Head 0 draws from the global torch RNG exactly as one
+    classifier does; the others are built with that RNG forked (the probe initialises on the host, so only the CPU
+    generator is drawn from) and then take head 0's state.  The RNG is left where one classifier leaves it, so the data
+    pipeline that draws from it next (erase seeds, samplers) sees the same stream for any number of heads."""
+    heads = [make_classifier()]
+    for _ in range(1, num_heads):
+        with torch.random.fork_rng(devices=[]):
+            clf = make_classifier()
+        clf.load_state_dict(heads[0].state_dict())
+        heads.append(clf)
+    return heads
+
+
+def train_heads(classifiers, multihead_kwargs, run_epoch, iterations_per_epoch, num_epochs, use_bfloat16,
+                resume_checkpoint, latest_path, log_file, device, rank, world_size, batch_size):
+    """The epoch loop of a multi-head run (both evaluation drivers): per head init_opt with its settings and its own
+    DistributedDataParallel wrapper; resume through load_multihead_checkpoint; one CSV row (epoch, head, loss, acc) per
+    head per epoch; checkpoint lists `classifiers` / `opts` / `scalers`.  run_epoch(training, heads) runs one epoch of
+    every head (heads: run_one_epoch's per-head keyword lists) and returns the per-head accuracies."""
+    ipe = iterations_per_epoch
+    opts, scalers, schedulers, wd_schedulers, wrapped = [], [], [], [], []
+    for clf, h in zip(classifiers, multihead_kwargs):
+        optimizer, scaler, scheduler, wd_scheduler = init_opt(
+            classifier=clf, wd=h['weight_decay'], final_wd=h['final_weight_decay'], start_lr=h['start_lr'],
+            ref_lr=h['lr'], final_lr=h['final_lr'], iterations_per_epoch=ipe, warmup=h['warmup'],
+            num_epochs=num_epochs, use_bfloat16=use_bfloat16)
+        opts.append(optimizer)
+        scalers.append(scaler)
+        schedulers.append(scheduler)
+        wd_schedulers.append(wd_scheduler)
+        wrapped.append(DistributedDataParallel(clf, static_graph=True))
+    logger.info(f'Training {len(wrapped)} attentive probes on one encoder pass per batch')
+
+    start_epoch = 0
+    if resume_checkpoint:
+        start_epoch = load_multihead_checkpoint(device=device, r_path=latest_path, classifiers=wrapped, opts=opts,
+                                                scalers=scalers, multihead_kwargs=multihead_kwargs)
+        for scheduler, wd_scheduler in zip(schedulers, wd_schedulers):
+            for _ in range(start_epoch * ipe):
+                scheduler.step()
+                wd_scheduler.step()
+
+    if rank == 0:
+        csv_logger = CSVLogger(log_file, ('%d', 'epoch'), ('%d', 'head'), ('%.5f', 'loss'), ('%.5f', 'acc'))
+    heads = dict(classifier=wrapped, scaler=scalers, optimizer=opts, scheduler=schedulers, wd_scheduler=wd_schedulers)
+    for epoch in range(start_epoch, num_epochs):
+        logger.info('Epoch %d' % (epoch + 1))
+        train_acc = run_epoch(True, heads)
+        val_acc = run_epoch(False, heads)
+        best = max(range(len(val_acc)), key=lambda k: val_acc[k])
+        logger.info('[%5d] best of %d heads: head %d train: %.3f%% test: %.3f%%'
+                    % (epoch + 1, len(val_acc), best, train_acc[best], val_acc[best]))
+        if rank == 0:
+            for k in range(len(wrapped)):
+                csv_logger.log(epoch + 1, k, train_acc[k], val_acc[k])
+            torch.save({
+                'classifiers': [clf.state_dict() for clf in wrapped],
+                'opts': [opt.state_dict() for opt in opts],
+                'scalers': [None if s is None else s.state_dict() for s in scalers],
+                'multihead_kwargs': multihead_kwargs,
+                'epoch': epoch + 1,
+                'batch_size': batch_size,
+                'world_size': world_size,
+            }, latest_path)
+
+
+def load_multihead_checkpoint(device, r_path, classifiers, opts, scalers, multihead_kwargs):
+    """Every head's classifier (module.-prefixed), optimizer and scaler state from a multi-head checkpoint; returns its
+    epoch.  A checkpoint whose resolved head settings differ from `multihead_kwargs`, or any failure, restarts at
+    epoch 0, as load_checkpoint does."""
+    try:
+        checkpoint = torch.load(r_path, map_location=torch.device('cpu'))
+        if checkpoint.get('multihead_kwargs') != multihead_kwargs:
+            raise ValueError(f"its heads {checkpoint.get('multihead_kwargs')} differ from the config's {multihead_kwargs}")
+        epoch = checkpoint['epoch']
+        for k, (clf, opt, scaler) in enumerate(zip(classifiers, opts, scalers)):
+            msg = clf.load_state_dict(checkpoint['classifiers'][k])
+            logger.info(f'loaded pretrained classifier {k} from epoch {epoch} with msg: {msg}')
+            opt.load_state_dict(checkpoint['opts'][k])
+            if scaler is not None:
+                scaler.load_state_dict(checkpoint['scalers'][k])
+        logger.info(f'loaded optimizers of {len(classifiers)} heads from epoch {epoch}')
+        logger.info(f'read-path: {r_path}')
+        del checkpoint
+    except Exception as e:
+        logger.info(f'Encountered exception when loading checkpoint {e}')
+        epoch = 0
+    return epoch
+
+
 def load_clips(data, device, data_loader):
     """data[0] (segments of views, collated) -> device.  uint8 frames from a loader whose dataset carries the GPU
     evaluation transform become the reference's views through vj_clip_views; training tickets of every segment go
@@ -247,15 +397,24 @@ def load_clips(data, device, data_loader):
 def run_one_epoch(device, training, encoder, classifier, scaler, optimizer, scheduler, wd_scheduler, data_loader,
                   use_bfloat16, num_spatial_views, num_temporal_views, attend_across_segments, fp16_autocast=False):
     """eval.py:298-380.  Without attend_across_segments every (view, segment) token set goes through the classifier on
-    its own; the probe's backward adds all of them into one flat gradient buffer, exchanged once across ranks."""
-    classifier.train(mode=training)
+    its own; the probe's backward adds all of them into one flat gradient buffer, exchanged once across ranks.
+
+    classifier, scaler, optimizer, scheduler and wd_scheduler may also be lists, one entry per head
+    (optimization.multihead_kwargs): the encoder then runs once per batch, each head runs the loop body on its output in
+    turn (forward, loss, accuracy, backward, its own scaler and optimizer step), and the per-head accuracies are
+    returned.  One head computes what one classifier does."""
+    multi = isinstance(classifier, (list, tuple))
+    heads = list(zip(*[x if multi else [x] for x in (classifier, scaler, optimizer, scheduler, wd_scheduler)]))
+    for clf, *_ in heads:
+        clf.train(mode=training)
     criterion = torch.nn.CrossEntropyLoss()
-    top1_meter = AverageMeter()
+    top1_meters = [AverageMeter() for _ in heads]
     for itr, data in enumerate(data_loader):
 
         if training:
-            scheduler.step()
-            wd_scheduler.step()
+            for *_, sched, wd_sched in heads:
+                sched.step()
+                wd_sched.step()
 
         # (without fp16_autocast no region: encoder and probe compute bf16 x bf16 -> fp32; see the module docstring)
         with loop_autocast(fp16_autocast, use_bfloat16):
@@ -265,49 +424,57 @@ def run_one_epoch(device, training, encoder, classifier, scaler, optimizer, sche
             batch_size = len(labels)
 
             with torch.no_grad():
-                outputs = encoder(clips, clip_indices)
-                if not training:
-                    if attend_across_segments:
-                        outputs = [classifier(o) for o in outputs]
-                    else:
-                        outputs = [[classifier(ost) for ost in os] for os in outputs]
-            if training:
+                tokens = encoder(clips, clip_indices)
+
+        for k, (clf, scaler, optimizer, _, _) in enumerate(heads):
+            # the classifier calls run in the same region as the encoder; validation under no_grad
+            with loop_autocast(fp16_autocast, use_bfloat16), torch.set_grad_enabled(training):
                 if attend_across_segments:
-                    outputs = [classifier(o) for o in outputs]
+                    outputs = [clf(o) for o in tokens]
                 else:
-                    outputs = [[classifier(ost) for ost in os] for os in outputs]
+                    outputs = [[clf(ost) for ost in os] for os in tokens]
 
-        if attend_across_segments:
-            loss = sum([criterion(o, labels) for o in outputs]) / len(outputs)
-        else:
-            loss = sum([sum([criterion(ost, labels) for ost in os]) for os in outputs]) / len(outputs) / len(outputs[0])
-        with torch.no_grad():
             if attend_across_segments:
-                outputs = sum([F.softmax(o, dim=1) for o in outputs]) / len(outputs)
+                loss = sum([criterion(o, labels) for o in outputs]) / len(outputs)
             else:
-                outputs = sum([sum([F.softmax(ost, dim=1) for ost in os]) for os in outputs]) / len(outputs) / len(outputs[0])
-            top1_acc = 100. * outputs.max(dim=1).indices.eq(labels).sum() / batch_size
-            top1_acc = float(AllReduce.apply(top1_acc))
-            top1_meter.update(top1_acc)
+                loss = (sum([sum([criterion(ost, labels) for ost in os]) for os in outputs])
+                        / len(outputs) / len(outputs[0]))
+            with torch.no_grad():
+                if attend_across_segments:
+                    outputs = sum([F.softmax(o, dim=1) for o in outputs]) / len(outputs)
+                else:
+                    outputs = (sum([sum([F.softmax(ost, dim=1) for ost in os]) for os in outputs])
+                               / len(outputs) / len(outputs[0]))
+                top1_acc = 100. * outputs.max(dim=1).indices.eq(labels).sum() / batch_size
+                top1_acc = float(AllReduce.apply(top1_acc))
+                top1_meters[k].update(top1_acc)
 
-        if training:
-            if use_bfloat16:
-                scaler.scale(loss).backward()
-                scaler.unscale_(optimizer)
-                torch.nn.utils.clip_grad_norm_(classifier.parameters(), 1.0)
-                scaler.step(optimizer)
-                scaler.update()
-            else:
-                loss.backward()
-                torch.nn.utils.clip_grad_norm_(classifier.parameters(), 1.0)
-                optimizer.step()
-            optimizer.zero_grad()
+            if training:
+                step_head(clf, scaler, optimizer, loss, use_bfloat16)
 
-        if itr % 20 == 0:
-            logger.info('[%5d] %.3f%% (loss: %.3f) [mem: %.2e]'
-                        % (itr, top1_meter.avg, loss, torch.cuda.max_memory_allocated() / 1024.**2))
+            if itr % 20 == 0:
+                logger.info(('[%5d] head %d: ' % (itr, k) if multi else '[%5d] ' % itr)
+                            + '%.3f%% (loss: %.3f) [mem: %.2e]'
+                            % (top1_meters[k].avg, loss, torch.cuda.max_memory_allocated() / 1024.**2))
 
-    return top1_meter.avg
+    accs = [m.avg for m in top1_meters]
+    return accs if multi else accs[0]
+
+
+def step_head(classifier, scaler, optimizer, loss, use_bfloat16):
+    """The reference's update (eval.py:358-370): GradScaler (use_bfloat16) or plain backward, clip to 1.0, AdamW step,
+    zero_grad.  With several heads each has its own scaler: an overflowing head skips its step and halves its scale."""
+    if use_bfloat16:
+        scaler.scale(loss).backward()
+        scaler.unscale_(optimizer)
+        torch.nn.utils.clip_grad_norm_(classifier.parameters(), 1.0)
+        scaler.step(optimizer)
+        scaler.update()
+    else:
+        loss.backward()
+        torch.nn.utils.clip_grad_norm_(classifier.parameters(), 1.0)
+        optimizer.step()
+    optimizer.zero_grad()
 
 
 def load_checkpoint(device, r_path, classifier, opt, scaler):

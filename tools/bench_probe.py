@@ -2,7 +2,13 @@
 """Frozen-evaluation probe training step (or validation step), clips/sec, at the ViT-L/16 K400 shape.
 
     python tools/bench_probe.py [--steps K] [--warmup W] [--batch B] [--mode train|val|image|xattn]
-                                [--dtype bfloat16|float16]
+                                [--dtype bfloat16|float16] [--heads 1,4,16]
+
+--heads (train, val, image) runs the evaluation loop with several probes on one encoder pass
+(optimization.multihead_kwargs): per step the encoder runs once, then every probe its forward (+ backward, GradScaler,
+clip and FlatAdamW step when training) in turn.  The listed probe counts alternate step by step in one session, and the
+JSON line gains one row per count: encoder ms, probe ms per probe and clips/s (images/s).  The top-level figures are
+those of the first count.
 
 --dtype float16 runs each step's encoder and classifier calls inside the reference's autocast(dtype=torch.float16)
 region (evals/video_classification_frozen/eval.py:323) with AttentiveClassifier(follow_autocast=True): fp16 encoder,
@@ -73,19 +79,20 @@ def run(args):
     n_seg, frames, crop, n_cls = 8, 16, 224, 400
     enc = vit_large(img_size=crop, num_frames=frames, tubelet_size=2, uniform_power=True).to(device).eval()
     encoder = ClipAggregation(enc, tubelet_size=2, attend_across_segments=True)
-    clf = AttentiveClassifier(embed_dim=enc.embed_dim, num_heads=enc.num_heads, depth=1, num_classes=n_cls,
-                              follow_autocast=args.dtype == "float16").to(device)
-    groups = [{"params": [p for n, p in clf.named_parameters() if ("bias" not in n) and (len(p.shape) != 1)]},
-              {"params": [p for n, p in clf.named_parameters() if ("bias" in n) or (len(p.shape) == 1)],
-               "WD_exclude": True, "weight_decay": 0}]
-    opt = FlatAdamW(groups, lr=1e-3, weight_decay=0.01)
-    scaler = FlatGradScaler()
+    heads = []
+    for _ in range(max(args.heads)):
+        clf = AttentiveClassifier(embed_dim=enc.embed_dim, num_heads=enc.num_heads, depth=1, num_classes=n_cls,
+                                  follow_autocast=args.dtype == "float16").to(device)
+        groups = [{"params": [p for n, p in clf.named_parameters() if ("bias" not in n) and (len(p.shape) != 1)]},
+                  {"params": [p for n, p in clf.named_parameters() if ("bias" in n) or (len(p.shape) == 1)],
+                   "WD_exclude": True, "weight_decay": 0}]
+        heads.append((clf, FlatAdamW(groups, lr=1e-3, weight_decay=0.01), FlatGradScaler()))
     crit = torch.nn.CrossEntropyLoss()
     g = torch.Generator(device="cpu").manual_seed(0)
     labels = torch.randint(0, n_cls, (B,), generator=g).to(device)
     clips = None
     ev = [torch.cuda.Event(enable_timing=True) for _ in range(4)]
-    enc_ms, probe_ms, aug_ms, aug_bytes = [], [], [], []
+    aug_ms, aug_bytes = [], []
     if args.uint8:          # the evaluation's training transform (RandAugment + erasing) on the GPU, from uint8 frames
         from jepa_b200.transforms import augment_batch, make_eval_transforms, pack_augment
         H0, W0 = 256, 340
@@ -97,7 +104,7 @@ def run(args):
     else:
         clips = [[torch.randn(B, 3, frames, crop, crop, generator=g).to(device)] for _ in range(n_seg)]
 
-    def step(timed):
+    def step(timed, n_heads):
         nonlocal clips
         if args.uint8:
             tickets = [tf(x) for x in host]              # host decisions, segment-major
@@ -111,33 +118,30 @@ def run(args):
         with _region(args):
             with torch.no_grad():
                 outputs = encoder(clips)
-            if timed:
-                ev[1].record()
-            logits = [clf(o) for o in outputs]
-        loss = sum([crit(o, labels) for o in logits]) / len(logits)
-        scaler.scale(loss).backward()
-        scaler.unscale_(opt)
-        clip_grad_norm_(clf, 1.0)
-        scaler.step(opt)
-        scaler.update()
-        opt.zero_grad()
+        if timed:
+            ev[1].record()
+        for clf, opt, scaler in heads[:n_heads]:        # the evaluation loop's per-head body on one encoder pass
+            with _region(args):
+                logits = [clf(o) for o in outputs]
+            loss = sum([crit(o, labels) for o in logits]) / len(logits)
+            scaler.scale(loss).backward()
+            scaler.unscale_(opt)
+            clip_grad_norm_(clf, 1.0)
+            scaler.step(opt)
+            scaler.update()
+            opt.zero_grad()
         if timed:
             ev[2].record()
 
-    for _ in range(args.warmup):
-        step(False)
-    torch.cuda.synchronize()
+    def measure():
+        return {"enc": ev[0].elapsed_time(ev[1]), "probe": ev[1].elapsed_time(ev[2]),
+                "aug": ev[3].elapsed_time(ev[0]) if args.uint8 else None}
+
     sampler = ClockSampler(0)
-    t0 = time.perf_counter()
-    for _ in range(args.steps):
-        step(True)
-        torch.cuda.synchronize()
-        enc_ms.append(ev[0].elapsed_time(ev[1]))
-        probe_ms.append(ev[1].elapsed_time(ev[2]))
-        if args.uint8:
-            aug_ms.append(ev[3].elapsed_time(ev[0]))
-    wall = time.perf_counter() - t0
+    res = _alternate(args, step, measure)
     clocks = sampler.stop()
+    times, wall = res[args.heads[0]]
+    enc_ms, probe_ms, aug_ms = ([t[k] for t in times] for k in ("enc", "probe", "aug"))
     extra = {}
     if args.uint8:
         ms = sorted(aug_ms)[len(aug_ms) // 2]
@@ -169,7 +173,43 @@ def run(args):
         "power_limit_w": float(card[1]) if len(card) > 1 else None,
         "clocks": clocks,
         **extra,
+        **_heads_rows(args, res, B, "enc", "probe", "clips/s"),
     }), flush=True)
+
+
+def _alternate(args, step, measure):
+    """Warm-up at every head count, then args.steps timed rounds, each running one step at every head count of
+    args.heads in turn (so that clock and thermal drift spread over all of them).  step(timed, n_heads) runs one step;
+    measure() reads its CUDA events after the synchronisation.  Returns {n_heads: (per-step measures, wall seconds)}."""
+    for n in args.heads:
+        for _ in range(args.warmup):
+            step(False, n)
+    torch.cuda.synchronize()
+    res = {n: ([], 0.0) for n in args.heads}
+    for _ in range(args.steps):
+        for n in args.heads:
+            t0 = time.perf_counter()
+            step(True, n)
+            torch.cuda.synchronize()
+            times, wall = res[n]
+            times.append(measure())
+            res[n] = (times, wall + time.perf_counter() - t0)
+    return res
+
+
+def _heads_rows(args, res, batch, enc_key, probe_key, unit):
+    """With --heads: one row per head count - encoder ms, probe ms per head (all heads' time / heads) and throughput."""
+    if not args.multi:
+        return {}
+    med = lambda v: sorted(v)[len(v) // 2]
+    rows = []
+    for n, (times, wall) in res.items():
+        rows.append({"heads": n, "encoder_fwd_ms": round(med([t[enc_key] for t in times]), 3),
+                     "probe_ms_per_head": round(med([t[probe_key] for t in times]) / n, 3),
+                     "probe_ms_all_heads": round(med([t[probe_key] for t in times]), 3),
+                     "value": round(batch * len(times) / wall, 2), "unit": unit})
+    return {"heads": rows, "heads_timing": "head counts alternate step by step in one session; per head = median time "
+                                           "of all heads' probe work after the encoder / heads; value = wall clock"}
 
 
 def _augment_bytes(tickets, pack_augment, out):
@@ -230,15 +270,14 @@ def run_val(args):
     for p in enc.parameters():          # frozen, as in the evaluation: the forward keeps no activations
         p.requires_grad = False
     encoder = ClipAggregation(enc, tubelet_size=2, attend_across_segments=True)
-    clf = AttentiveClassifier(embed_dim=enc.embed_dim, num_heads=enc.num_heads, depth=1, num_classes=n_cls,
-                              follow_autocast=args.dtype == "float16").to(device).eval()
+    clfs = [AttentiveClassifier(embed_dim=enc.embed_dim, num_heads=enc.num_heads, depth=1, num_classes=n_cls,
+                                follow_autocast=args.dtype == "float16").to(device).eval() for _ in range(max(args.heads))]
     g = torch.Generator().manual_seed(0)
     segments = [torch.randint(0, 256, (B, frames, H0, W0, 3), dtype=torch.uint8, generator=g).pin_memory()
                 for _ in range(n_seg)]
-    ev = [torch.cuda.Event(enable_timing=True) for _ in range(3)]
-    view_ms, enc_ms = [], []
+    ev = [torch.cuda.Event(enable_timing=True) for _ in range(4)]
 
-    def step(timed):
+    def step(timed, n_heads):
         if timed:
             ev[0].record()
         with torch.no_grad():
@@ -246,24 +285,26 @@ def run_val(args):
             if timed:
                 ev[1].record()
             with _region(args):
-                outputs = [clf(o) for o in encoder(clips)]
-            probs = sum([F.softmax(o, dim=1) for o in outputs]) / len(outputs)
+                tokens = encoder(clips)
+            if timed:
+                ev[3].record()
+            for clf in clfs[:n_heads]:
+                with _region(args):
+                    outputs = [clf(o) for o in tokens]
+                probs = sum([F.softmax(o, dim=1) for o in outputs]) / len(outputs)
         if timed:
             ev[2].record()
         return probs
 
-    for _ in range(args.warmup):
-        step(False)
-    torch.cuda.synchronize()
+    def measure():
+        return {"views": ev[0].elapsed_time(ev[1]), "enc_probe": ev[1].elapsed_time(ev[2]),
+                "enc": ev[1].elapsed_time(ev[3]), "probe": ev[3].elapsed_time(ev[2])}
+
     sampler = ClockSampler(0)
-    t0 = time.perf_counter()
-    for _ in range(args.steps):
-        step(True)
-        torch.cuda.synchronize()
-        view_ms.append(ev[0].elapsed_time(ev[1]))
-        enc_ms.append(ev[1].elapsed_time(ev[2]))
-    wall = time.perf_counter() - t0
+    res = _alternate(args, step, measure)
     clocks = sampler.stop()
+    times, wall = res[args.heads[0]]
+    view_ms, enc_ms = [t["views"] for t in times], [t["enc_probe"] for t in times]
 
     # vj_clip_views alone, frames already on the device
     clips_u8 = [c for seg in segments for c in seg.unbind(0)]
@@ -303,6 +344,7 @@ def run_val(args):
         "gpu": card[0] if card else None,
         "power_limit_w": float(card[1]) if len(card) > 1 else None,
         "clocks": clocks,
+        **_heads_rows(args, res, B, "enc", "probe", "clips/s"),
     }), flush=True)
 
 
@@ -320,13 +362,14 @@ def run_image(args):
     enc = vit_large(img_size=crop, num_frames=frames, tubelet_size=2, uniform_power=True).to(device).eval()
     for p in enc.parameters():
         p.requires_grad = False
-    clf = AttentiveClassifier(embed_dim=enc.embed_dim, num_heads=enc.num_heads, depth=1, num_classes=n_cls,
-                              follow_autocast=args.dtype == "float16").to(device)
-    groups = [{"params": [p for n, p in clf.named_parameters() if ("bias" not in n) and (len(p.shape) != 1)]},
-              {"params": [p for n, p in clf.named_parameters() if ("bias" in n) or (len(p.shape) == 1)],
-               "WD_exclude": True, "weight_decay": 0}]
-    opt = FlatAdamW(groups, lr=1e-3, weight_decay=0.01)
-    scaler = FlatGradScaler()
+    heads = []
+    for _ in range(max(args.heads)):
+        clf = AttentiveClassifier(embed_dim=enc.embed_dim, num_heads=enc.num_heads, depth=1, num_classes=n_cls,
+                                  follow_autocast=args.dtype == "float16").to(device)
+        groups = [{"params": [p for n, p in clf.named_parameters() if ("bias" not in n) and (len(p.shape) != 1)]},
+                  {"params": [p for n, p in clf.named_parameters() if ("bias" in n) or (len(p.shape) == 1)],
+                   "WD_exclude": True, "weight_decay": 0}]
+        heads.append((clf, FlatAdamW(groups, lr=1e-3, weight_decay=0.01), FlatGradScaler()))
     crit = torch.nn.CrossEntropyLoss()
     g = torch.Generator(device="cpu").manual_seed(0)
     labels = torch.randint(0, n_cls, (B,), generator=g).to(device)
@@ -334,9 +377,9 @@ def run_image(args):
     host = [torch.randint(0, 256, (H0, W0, 3), dtype=torch.uint8, generator=g).numpy() for _ in range(B)]
     imgs = None if args.uint8 else torch.randn(B, 3, crop, crop, generator=g).to(device)
     ev = [torch.cuda.Event(enable_timing=True) for _ in range(4)]
-    enc_ms, probe_ms, tf_ms, host_ms = [], [], [], []
+    host_ms = []
 
-    def step(timed):
+    def step(timed, n_heads):
         nonlocal imgs
         if args.uint8:
             t0 = time.perf_counter()
@@ -350,33 +393,31 @@ def run_image(args):
         with _region(args):
             with torch.no_grad():
                 outputs = enc(imgs.unsqueeze(2).repeat(1, 1, frames, 1, 1))
-            if timed:
-                ev[1].record()
-            logits = clf(outputs)
-        loss = crit(logits, labels)
-        scaler.scale(loss).backward()
-        scaler.unscale_(opt)
-        clip_grad_norm_(clf, 1.0)
-        scaler.step(opt)
-        scaler.update()
-        opt.zero_grad()
+        if timed:
+            ev[1].record()
+        for clf, opt, scaler in heads[:n_heads]:        # the evaluation loop's per-head body on one encoder pass
+            with _region(args):
+                logits = clf(outputs)
+            loss = crit(logits, labels)
+            scaler.scale(loss).backward()
+            scaler.unscale_(opt)
+            clip_grad_norm_(clf, 1.0)
+            scaler.step(opt)
+            scaler.update()
+            opt.zero_grad()
         if timed:
             ev[2].record()
 
-    for _ in range(args.warmup):
-        step(False)
-    torch.cuda.synchronize()
+    def measure():
+        return {"enc": ev[0].elapsed_time(ev[1]), "probe": ev[1].elapsed_time(ev[2]),
+                "tf": ev[3].elapsed_time(ev[0]) if args.uint8 else None}
+
     sampler = ClockSampler(0)
-    t0 = time.perf_counter()
-    for _ in range(args.steps):
-        step(True)
-        torch.cuda.synchronize()
-        enc_ms.append(ev[0].elapsed_time(ev[1]))
-        probe_ms.append(ev[1].elapsed_time(ev[2]))
-        if args.uint8:
-            tf_ms.append(ev[3].elapsed_time(ev[0]))
-    wall = time.perf_counter() - t0
+    res = _alternate(args, step, measure)
     clocks = sampler.stop()
+    times, wall = res[args.heads[0]]
+    enc_ms, probe_ms = [t["enc"] for t in times], [t["probe"] for t in times]
+    tf_ms = [t["tf"] for t in times] if args.uint8 else []
 
     # the kernels alone, on staged batches already on the device
     images = [torch.from_numpy(x) for x in host]
@@ -425,6 +466,7 @@ def run_image(args):
         "gpu": card[0] if card else None,
         "power_limit_w": float(card[1]) if len(card) > 1 else None,
         "clocks": clocks,
+        **_heads_rows(args, res, B, "enc", "probe", "images/s"),
     }), flush=True)
 
 
@@ -531,7 +573,17 @@ def main():
                     help="float16: encoder and probe under the reference's autocast(float16) region")
     ap.add_argument("--uint8", action="store_true",
                     help="train / image mode: uint8 frames / images through the GPU training transform")
+    ap.add_argument("--heads", default=None,
+                    help="train / val / image mode: comma-separated probe counts trained (validated) on one encoder "
+                         "pass, e.g. 1,4,16, alternated step by step; reports encoder ms, probe ms per head and "
+                         "throughput for each")
     args = ap.parse_args()
+    args.multi = args.heads is not None
+    args.heads = [int(n) for n in args.heads.split(",")] if args.multi else [1]
+    if any(n < 1 for n in args.heads) or len(set(args.heads)) != len(args.heads):
+        ap.error("--heads: distinct positive head counts")
+    if args.multi and args.mode == "xattn":
+        ap.error("--heads applies to --mode train, val and image")
     if args.mode == "image":
         run_image(args)
         return
