@@ -3,7 +3,8 @@
 Same config keys, log lines, CSV columns and checkpoint dictionary as the reference (evals/image_classification_frozen/
 eval.py:63-521): a video encoder from pre-training sees each image repeated `frames_per_clip` times (a forward pre-hook,
 reference :451-456), and the attentive probe trains on its tokens with one classifier call per step.  The optimizer,
-checkpoint and encoder-loading helpers are the video evaluation's (the reference has identical copies).
+checkpoint and encoder-loading helpers, the epoch loop (train_heads) and the batch loop (run_head_loop) are the video
+evaluation's (the reference has identical copies of the helpers); run_one_epoch supplies the image batch and loss.
 
 The reference autocasts the loop body to fp16 (eval.py:284, `autocast(dtype=torch.float16, enabled=use_bfloat16)`).
 By default this loop opens no autocast region, so encoder and probe compute bf16 x bf16 -> fp32, and `use_bfloat16`
@@ -12,7 +13,7 @@ reference does and builds the classifier to follow it, exactly as in the video e
 `use_bfloat16: true`, bf16 throughout with `use_bfloat16: false`.  There is no fp32 path.
 
 `optimization.multihead_kwargs` trains several probes on one encoder pass per batch, with the video evaluation's parser,
-head construction, epoch loop, checkpoint and CSV layout (read_multihead_kwargs, build_heads, train_heads).
+head construction, checkpoint and CSV layout (read_multihead_kwargs, build_heads, train_heads).
 """
 import os
 
@@ -28,15 +29,15 @@ import pprint
 import numpy as np
 import torch
 import torch.multiprocessing as mp
+import torch.nn.functional as F
 
 import src.models.vision_transformer as vit
-from evals.video_classification_frozen.eval import (build_heads, init_opt, load_checkpoint, load_pretrained,
-                                                    loop_autocast, read_fp16_autocast, read_multihead_kwargs,
-                                                    require_cuda, step_head, train_heads)
+from evals.video_classification_frozen.eval import (  # noqa: F401  (the helpers both evaluations share)
+    build_heads, init_opt, load_checkpoint, load_pretrained, loop_autocast, one_head, read_fp16_autocast,
+    read_multihead_kwargs, require_cuda, run_head_loop, step_head, train_heads)
 from src.datasets.data_manager import init_data
 from src.models.attentive_pooler import AttentiveClassifier
-from src.utils.distributed import AllReduce, DistributedDataParallel, init_distributed
-from src.utils.logging import AverageMeter, CSVLogger
+from src.utils.distributed import init_distributed
 
 logging.basicConfig()
 logger = logging.getLogger()
@@ -107,9 +108,6 @@ def main(args_eval, resume_preempt=False):
     log_file = os.path.join(folder, f'{tag}_r{rank}.csv')
     latest_path = os.path.join(folder, f'{tag}-latest.pth.tar')
 
-    if rank == 0 and multihead_kwargs is None:
-        csv_logger = CSVLogger(log_file, ('%d', 'epoch'), ('%.5f', 'loss'), ('%.5f', 'acc'))
-
     encoder = init_model(crop_size=resolution, device=device, pretrained=pretrained_path, model_name=model_name,
                          patch_size=patch_size, frames_per_clip=frames_per_clip, tubelet_size=tubelet_size,
                          uniform_power=uniform_power, checkpoint_key=checkpoint_key, use_SiLU=use_SiLU,
@@ -118,10 +116,10 @@ def main(args_eval, resume_preempt=False):
     for p in encoder.parameters():
         p.requires_grad = False
 
+    settings = multihead_kwargs or [one_head(wd, start_lr, lr, final_lr, warmup)]
     classifiers = build_heads(lambda: AttentiveClassifier(embed_dim=encoder.embed_dim, num_heads=encoder.num_heads,
                                                           depth=1, num_classes=num_classes,
-                                                          follow_autocast=fp16_autocast).to(device),
-                              1 if multihead_kwargs is None else len(multihead_kwargs))
+                                                          follow_autocast=fp16_autocast).to(device), len(settings))
 
     train_loader = make_dataloader(dataset_name=dataset_name, root_path=root_path, resolution=resolution,
                                    image_folder=image_folder, batch_size=batch_size, world_size=world_size, rank=rank,
@@ -132,105 +130,34 @@ def main(args_eval, resume_preempt=False):
     ipe = len(train_loader)
     logger.info(f'Dataloader created... iterations per epoch: {ipe}')
 
-    if multihead_kwargs is not None:
-        def run_epoch(training, heads):
-            return run_one_epoch(device=device, training=training, encoder=encoder,
-                                 data_loader=train_loader if training else val_loader, use_bfloat16=use_bfloat16,
-                                 fp16_autocast=fp16_autocast, **heads)
-        train_heads(classifiers, multihead_kwargs, run_epoch, iterations_per_epoch=ipe, num_epochs=num_epochs,
-                    use_bfloat16=use_bfloat16, resume_checkpoint=resume_checkpoint, latest_path=latest_path,
-                    log_file=log_file, device=device, rank=rank, world_size=world_size, batch_size=batch_size)
-        return
-
-    classifier = classifiers[0]
-    optimizer, scaler, scheduler, wd_scheduler = init_opt(
-        classifier=classifier, wd=wd, start_lr=start_lr, ref_lr=lr, final_lr=final_lr, iterations_per_epoch=ipe,
-        warmup=warmup, num_epochs=num_epochs, use_bfloat16=use_bfloat16)
-    classifier = DistributedDataParallel(classifier, static_graph=True)
-
-    start_epoch = 0
-    if resume_checkpoint:
-        classifier, optimizer, scaler, start_epoch = load_checkpoint(device=device, r_path=latest_path,
-                                                                     classifier=classifier, opt=optimizer, scaler=scaler)
-        for _ in range(start_epoch * ipe):
-            scheduler.step()
-            wd_scheduler.step()
-
-    def save_checkpoint(epoch):
-        save_dict = {
-            'classifier': classifier.state_dict(),
-            'opt': optimizer.state_dict(),
-            'scaler': None if scaler is None else scaler.state_dict(),
-            'epoch': epoch,
-            'batch_size': batch_size,
-            'world_size': world_size,
-            'lr': lr,
-        }
-        if rank == 0:
-            torch.save(save_dict, latest_path)
-
-    for epoch in range(start_epoch, num_epochs):
-        logger.info('Epoch %d' % (epoch + 1))
-        train_acc = run_one_epoch(device=device, training=True, encoder=encoder, classifier=classifier, scaler=scaler,
-                                  optimizer=optimizer, scheduler=scheduler, wd_scheduler=wd_scheduler,
-                                  data_loader=train_loader, use_bfloat16=use_bfloat16, fp16_autocast=fp16_autocast)
-        val_acc = run_one_epoch(device=device, training=False, encoder=encoder, classifier=classifier, scaler=scaler,
-                                optimizer=optimizer, scheduler=scheduler, wd_scheduler=wd_scheduler,
-                                data_loader=val_loader, use_bfloat16=use_bfloat16, fp16_autocast=fp16_autocast)
-        logger.info('[%5d] train: %.3f%% test: %.3f%%' % (epoch + 1, train_acc, val_acc))
-        if rank == 0:
-            csv_logger.log(epoch + 1, train_acc, val_acc)
-        save_checkpoint(epoch + 1)
+    def run_epoch(training, heads):
+        return run_one_epoch(device=device, training=training, encoder=encoder,
+                             data_loader=train_loader if training else val_loader, use_bfloat16=use_bfloat16,
+                             fp16_autocast=fp16_autocast, **heads)
+    train_heads(classifiers, settings, run_epoch, multihead=multihead_kwargs is not None, iterations_per_epoch=ipe,
+                num_epochs=num_epochs, use_bfloat16=use_bfloat16, resume_checkpoint=resume_checkpoint,
+                latest_path=latest_path, log_file=log_file, device=device, rank=rank, world_size=world_size,
+                batch_size=batch_size)
 
 
 def run_one_epoch(device, training, encoder, classifier, scaler, optimizer, scheduler, wd_scheduler, data_loader,
                   use_bfloat16, fp16_autocast=False):
-    """eval.py:262-317: one classifier call per step.  classifier, scaler, optimizer, scheduler and wd_scheduler may be
-    lists, one entry per head, as in the video evaluation's run_one_epoch: one encoder pass per batch, then each head's
-    loop body in turn; the per-head accuracies are returned."""
-    multi = isinstance(classifier, (list, tuple))
-    heads = list(zip(*[x if multi else [x] for x in (classifier, scaler, optimizer, scheduler, wd_scheduler)]))
-    for clf, *_ in heads:
-        clf.train(mode=training)
-    criterion = torch.nn.CrossEntropyLoss()
-    top1_meters = [AverageMeter() for _ in heads]
-    for itr, data in enumerate(data_loader):
+    """eval.py:262-317: one classifier call per step, the cross-entropy of its logits as the loss and their argmax
+    (not that of their softmax, whose rounding can tie) as the top-1.  The loop itself, also for per-head lists, is the
+    video evaluation's run_head_loop."""
+    def encode(data):
+        if isinstance(data[0], list):       # uint8 image tickets: the transform's pixel work runs on the GPU
+            imgs = data_loader.dataset.transform.batch(data[0], device)
+        else:
+            imgs = data[0].to(device)
+        labels = data[1].to(device)
+        return encoder(imgs), labels, len(imgs)
 
-        if training:
-            for *_, sched, wd_sched in heads:
-                sched.step()
-                wd_sched.step()
+    def loss_and_scores(outputs, labels):
+        return F.cross_entropy(outputs, labels), outputs
 
-        # (without fp16_autocast no region: encoder and probe compute bf16 x bf16 -> fp32; see the module docstring)
-        with loop_autocast(fp16_autocast, use_bfloat16):
-            if isinstance(data[0], list):       # uint8 image tickets: the transform's pixel work runs on the GPU
-                imgs = data_loader.dataset.transform.batch(data[0], device)
-            else:
-                imgs = data[0].to(device)
-            labels = data[1].to(device)
-            with torch.no_grad():
-                tokens = encoder(imgs)
-
-        for k, (clf, scaler, optimizer, _, _) in enumerate(heads):
-            # the classifier call runs in the same region as the encoder; validation under no_grad
-            with loop_autocast(fp16_autocast, use_bfloat16), torch.set_grad_enabled(training):
-                outputs = clf(tokens)
-
-            loss = criterion(outputs, labels)
-            top1_acc = 100. * outputs.max(dim=1).indices.eq(labels).sum() / len(imgs)
-            top1_acc = float(AllReduce.apply(top1_acc))
-            top1_meters[k].update(top1_acc)
-
-            if training:
-                step_head(clf, scaler, optimizer, loss, use_bfloat16)
-
-            if itr % 20 == 0:
-                logger.info(('[%5d] head %d: ' % (itr, k) if multi else '[%5d] ' % itr)
-                            + '%.3f%% (loss: %.3f) [mem: %.2e]'
-                            % (top1_meters[k].avg, loss, torch.cuda.max_memory_allocated() / 1024.**2))
-
-    accs = [m.avg for m in top1_meters]
-    return accs if multi else accs[0]
+    return run_head_loop(training, classifier, scaler, optimizer, scheduler, wd_scheduler, data_loader, use_bfloat16,
+                         fp16_autocast, encode, loss_and_scores)
 
 
 def make_dataloader(dataset_name, root_path, image_folder, batch_size, world_size, rank, resolution=224, training=False,

@@ -19,8 +19,9 @@ computes in bf16 as by default.  There is no fp32 path.
 
 `optimization.multihead_kwargs` (a list of per-head lr / start_lr / final_lr / weight_decay / final_weight_decay /
 warmup, read by read_multihead_kwargs) trains several probes ("heads") on one encoder pass per batch: every head starts
-from the same weights and has its own optimizer, schedules, GradScaler and gradient exchange (train_heads).  Without the
-key the driver trains one classifier with the reference's checkpoint, CSV and log lines.
+from the same weights and has its own optimizer, schedules, GradScaler and gradient exchange.  Without the key the
+driver trains one classifier with the reference's checkpoint, CSV and log lines.  Both cases, and the image evaluation,
+run the same epoch loop (train_heads) and batch loop (run_head_loop).
 """
 import collections.abc
 import contextlib
@@ -135,9 +136,6 @@ def main(args_eval, resume_preempt=False):
     log_file = os.path.join(folder, f'{tag}_r{rank}.csv')
     latest_path = os.path.join(folder, f'{tag}-latest.pth.tar')
 
-    if rank == 0 and multihead_kwargs is None:
-        csv_logger = CSVLogger(log_file, ('%d', 'epoch'), ('%.5f', 'loss'), ('%.5f', 'acc'))
-
     # -- pretrained encoder (frozen)
     encoder = init_model(crop_size=resolution, device=device, pretrained=pretrained_path, model_name=model_name,
                          patch_size=patch_size, tubelet_size=tubelet_size, frames_per_clip=pretrain_frames_per_clip,
@@ -157,10 +155,10 @@ def main(args_eval, resume_preempt=False):
     for p in encoder.parameters():
         p.requires_grad = False
 
+    settings = multihead_kwargs or [one_head(wd, start_lr, lr, final_lr, warmup)]
     classifiers = build_heads(lambda: AttentiveClassifier(embed_dim=encoder.embed_dim, num_heads=encoder.num_heads,
                                                           depth=1, num_classes=num_classes,
-                                                          follow_autocast=fp16_autocast).to(device),
-                              1 if multihead_kwargs is None else len(multihead_kwargs))
+                                                          follow_autocast=fp16_autocast).to(device), len(settings))
 
     train_loader = make_dataloader(dataset_type=dataset_type, root_path=train_data_path, resolution=resolution,
                                    frames_per_clip=eval_frames_per_clip, frame_step=eval_frame_step,
@@ -178,63 +176,17 @@ def main(args_eval, resume_preempt=False):
     ipe = len(train_loader)
     logger.info(f'Dataloader created... iterations per epoch: {ipe}')
 
-    if multihead_kwargs is not None:
-        def run_epoch(training, heads):
-            return run_one_epoch(device=device, training=training,
-                                 num_temporal_views=eval_num_segments if (attend_across_segments or not training) else 1,
-                                 attend_across_segments=attend_across_segments,
-                                 num_spatial_views=1 if training else eval_num_views_per_segment, encoder=encoder,
-                                 data_loader=train_loader if training else val_loader, use_bfloat16=use_bfloat16,
-                                 fp16_autocast=fp16_autocast, **heads)
-        train_heads(classifiers, multihead_kwargs, run_epoch, iterations_per_epoch=ipe, num_epochs=num_epochs,
-                    use_bfloat16=use_bfloat16, resume_checkpoint=resume_checkpoint, latest_path=latest_path,
-                    log_file=log_file, device=device, rank=rank, world_size=world_size, batch_size=batch_size)
-        return
-
-    classifier = classifiers[0]
-    optimizer, scaler, scheduler, wd_scheduler = init_opt(
-        classifier=classifier, wd=wd, start_lr=start_lr, ref_lr=lr, final_lr=final_lr, iterations_per_epoch=ipe,
-        warmup=warmup, num_epochs=num_epochs, use_bfloat16=use_bfloat16)
-    classifier = DistributedDataParallel(classifier, static_graph=True)
-
-    start_epoch = 0
-    if resume_checkpoint:
-        classifier, optimizer, scaler, start_epoch = load_checkpoint(device=device, r_path=latest_path,
-                                                                     classifier=classifier, opt=optimizer, scaler=scaler)
-        for _ in range(start_epoch * ipe):
-            scheduler.step()
-            wd_scheduler.step()
-
-    def save_checkpoint(epoch):
-        save_dict = {
-            'classifier': classifier.state_dict(),
-            'opt': optimizer.state_dict(),
-            'scaler': None if scaler is None else scaler.state_dict(),
-            'epoch': epoch,
-            'batch_size': batch_size,
-            'world_size': world_size,
-            'lr': lr,
-        }
-        if rank == 0:
-            torch.save(save_dict, latest_path)
-
-    for epoch in range(start_epoch, num_epochs):
-        logger.info('Epoch %d' % (epoch + 1))
-        train_acc = run_one_epoch(device=device, training=True,
-                                  num_temporal_views=eval_num_segments if attend_across_segments else 1,
-                                  attend_across_segments=attend_across_segments, num_spatial_views=1, encoder=encoder,
-                                  classifier=classifier, scaler=scaler, optimizer=optimizer, scheduler=scheduler,
-                                  wd_scheduler=wd_scheduler, data_loader=train_loader, use_bfloat16=use_bfloat16,
-                                  fp16_autocast=fp16_autocast)
-        val_acc = run_one_epoch(device=device, training=False, num_temporal_views=eval_num_segments,
-                                attend_across_segments=attend_across_segments,
-                                num_spatial_views=eval_num_views_per_segment, encoder=encoder, classifier=classifier,
-                                scaler=scaler, optimizer=optimizer, scheduler=scheduler, wd_scheduler=wd_scheduler,
-                                data_loader=val_loader, use_bfloat16=use_bfloat16, fp16_autocast=fp16_autocast)
-        logger.info('[%5d] train: %.3f%% test: %.3f%%' % (epoch + 1, train_acc, val_acc))
-        if rank == 0:
-            csv_logger.log(epoch + 1, train_acc, val_acc)
-        save_checkpoint(epoch + 1)
+    def run_epoch(training, heads):
+        return run_one_epoch(device=device, training=training,
+                             num_temporal_views=eval_num_segments if (attend_across_segments or not training) else 1,
+                             attend_across_segments=attend_across_segments,
+                             num_spatial_views=1 if training else eval_num_views_per_segment, encoder=encoder,
+                             data_loader=train_loader if training else val_loader, use_bfloat16=use_bfloat16,
+                             fp16_autocast=fp16_autocast, **heads)
+    train_heads(classifiers, settings, run_epoch, multihead=multihead_kwargs is not None, iterations_per_epoch=ipe,
+                num_epochs=num_epochs, use_bfloat16=use_bfloat16, resume_checkpoint=resume_checkpoint,
+                latest_path=latest_path, log_file=log_file, device=device, rank=rank, world_size=world_size,
+                batch_size=batch_size)
 
 
 def read_fp16_autocast(args_opt):
@@ -289,6 +241,12 @@ def read_multihead_kwargs(args_opt):
     return heads
 
 
+def one_head(wd, start_lr, lr, final_lr, warmup):
+    """The settings of a run without multihead_kwargs: its one classifier takes the top-level `optimization` values as
+    the reference passes them to init_opt - unconverted and unchecked - with init_opt's final weight decay of 1e-6."""
+    return dict(lr=lr, start_lr=start_lr, final_lr=final_lr, weight_decay=wd, final_weight_decay=1e-6, warmup=warmup)
+
+
 def build_heads(make_classifier, num_heads):
     """num_heads classifiers with equal initial weights.  Head 0 draws from the global torch RNG exactly as one
     classifier does; the others are built with that RNG forked (the probe initialises on the host, so only the CPU
@@ -303,15 +261,18 @@ def build_heads(make_classifier, num_heads):
     return heads
 
 
-def train_heads(classifiers, multihead_kwargs, run_epoch, iterations_per_epoch, num_epochs, use_bfloat16,
+def train_heads(classifiers, settings, run_epoch, multihead, iterations_per_epoch, num_epochs, use_bfloat16,
                 resume_checkpoint, latest_path, log_file, device, rank, world_size, batch_size):
-    """The epoch loop of a multi-head run (both evaluation drivers): per head init_opt with its settings and its own
-    DistributedDataParallel wrapper; resume through load_multihead_checkpoint; one CSV row (epoch, head, loss, acc) per
-    head per epoch; checkpoint lists `classifiers` / `opts` / `scalers`.  run_epoch(training, heads) runs one epoch of
-    every head (heads: run_one_epoch's per-head keyword lists) and returns the per-head accuracies."""
+    """The epoch loop of both evaluation drivers: per head init_opt with its settings (a dict of MULTIHEAD_FIELDS) and a
+    DistributedDataParallel wrapper, resume, then per epoch run_epoch(training, heads) (heads: run_one_epoch's per-head
+    keywords, returning the accuracies), a log line, CSV rows and the checkpoint.  Without `multihead` the one head
+    keeps the reference's layout: run_one_epoch's single-classifier form, CSV `epoch,loss,acc`, checkpoint `classifier` /
+    `opt` / `scaler` / ... / `lr`.  With it: CSV `epoch,head,loss,acc`, checkpoint lists `classifiers` / `opts` /
+    `scalers` with the resolved `multihead_kwargs`, and the epoch line names the head with the best validation
+    accuracy."""
     ipe = iterations_per_epoch
     opts, scalers, schedulers, wd_schedulers, wrapped = [], [], [], [], []
-    for clf, h in zip(classifiers, multihead_kwargs):
+    for clf, h in zip(classifiers, settings):
         optimizer, scaler, scheduler, wd_scheduler = init_opt(
             classifier=clf, wd=h['weight_decay'], final_wd=h['final_weight_decay'], start_lr=h['start_lr'],
             ref_lr=h['lr'], final_lr=h['final_lr'], iterations_per_epoch=ipe, warmup=h['warmup'],
@@ -321,57 +282,69 @@ def train_heads(classifiers, multihead_kwargs, run_epoch, iterations_per_epoch, 
         schedulers.append(scheduler)
         wd_schedulers.append(wd_scheduler)
         wrapped.append(DistributedDataParallel(clf, static_graph=True))
-    logger.info(f'Training {len(wrapped)} attentive probes on one encoder pass per batch')
+    if multihead:
+        logger.info(f'Training {len(wrapped)} attentive probes on one encoder pass per batch')
 
     start_epoch = 0
     if resume_checkpoint:
         start_epoch = load_multihead_checkpoint(device=device, r_path=latest_path, classifiers=wrapped, opts=opts,
-                                                scalers=scalers, multihead_kwargs=multihead_kwargs)
+                                                scalers=scalers, multihead_kwargs=settings if multihead else None)
         for scheduler, wd_scheduler in zip(schedulers, wd_schedulers):
             for _ in range(start_epoch * ipe):
                 scheduler.step()
                 wd_scheduler.step()
 
+    head_column = [('%d', 'head')] if multihead else []
     if rank == 0:
-        csv_logger = CSVLogger(log_file, ('%d', 'epoch'), ('%d', 'head'), ('%.5f', 'loss'), ('%.5f', 'acc'))
+        csv_logger = CSVLogger(log_file, ('%d', 'epoch'), *head_column, ('%.5f', 'loss'), ('%.5f', 'acc'))
     heads = dict(classifier=wrapped, scaler=scalers, optimizer=opts, scheduler=schedulers, wd_scheduler=wd_schedulers)
+    if not multihead:
+        heads = {key: v[0] for key, v in heads.items()}
     for epoch in range(start_epoch, num_epochs):
         logger.info('Epoch %d' % (epoch + 1))
         train_acc = run_epoch(True, heads)
         val_acc = run_epoch(False, heads)
+        if not multihead:
+            train_acc, val_acc = [train_acc], [val_acc]
         best = max(range(len(val_acc)), key=lambda k: val_acc[k])
-        logger.info('[%5d] best of %d heads: head %d train: %.3f%% test: %.3f%%'
-                    % (epoch + 1, len(val_acc), best, train_acc[best], val_acc[best]))
+        logger.info(('[%5d] best of %d heads: head %d ' % (epoch + 1, len(val_acc), best) if multihead
+                     else '[%5d] ' % (epoch + 1))
+                    + 'train: %.3f%% test: %.3f%%' % (train_acc[best], val_acc[best]))
         if rank == 0:
             for k in range(len(wrapped)):
-                csv_logger.log(epoch + 1, k, train_acc[k], val_acc[k])
-            torch.save({
-                'classifiers': [clf.state_dict() for clf in wrapped],
-                'opts': [opt.state_dict() for opt in opts],
-                'scalers': [None if s is None else s.state_dict() for s in scalers],
-                'multihead_kwargs': multihead_kwargs,
-                'epoch': epoch + 1,
-                'batch_size': batch_size,
-                'world_size': world_size,
-            }, latest_path)
+                csv_logger.log(epoch + 1, *([k] if multihead else []), train_acc[k], val_acc[k])
+            scaler_states = [None if s is None else s.state_dict() for s in scalers]
+            if multihead:
+                checkpoint = {'classifiers': [c.state_dict() for c in wrapped], 'opts': [o.state_dict() for o in opts],
+                              'scalers': scaler_states, 'multihead_kwargs': settings,
+                              'epoch': epoch + 1, 'batch_size': batch_size, 'world_size': world_size}
+            else:
+                checkpoint = {'classifier': wrapped[0].state_dict(), 'opt': opts[0].state_dict(),
+                              'scaler': scaler_states[0], 'epoch': epoch + 1, 'batch_size': batch_size,
+                              'world_size': world_size, 'lr': settings[0]['lr']}
+            torch.save(checkpoint, latest_path)
 
 
 def load_multihead_checkpoint(device, r_path, classifiers, opts, scalers, multihead_kwargs):
-    """Every head's classifier (module.-prefixed), optimizer and scaler state from a multi-head checkpoint; returns its
-    epoch.  A checkpoint whose resolved head settings differ from `multihead_kwargs`, or any failure, restarts at
-    epoch 0, as load_checkpoint does."""
+    """Every head's classifier (module.-prefixed), optimizer and scaler state; returns the checkpoint's epoch, or 0
+    after any failure.  multihead_kwargs None reads the reference's one-classifier layout (eval.py:383-411: `classifier`,
+    `opt`, `scaler`); a list reads the multi-head layout (`classifiers`, `opts`, `scalers`), and a checkpoint whose
+    resolved head settings differ from it is not loaded."""
+    multihead = multihead_kwargs is not None
     try:
         checkpoint = torch.load(r_path, map_location=torch.device('cpu'))
-        if checkpoint.get('multihead_kwargs') != multihead_kwargs:
+        if multihead and checkpoint.get('multihead_kwargs') != multihead_kwargs:
             raise ValueError(f"its heads {checkpoint.get('multihead_kwargs')} differ from the config's {multihead_kwargs}")
         epoch = checkpoint['epoch']
         for k, (clf, opt, scaler) in enumerate(zip(classifiers, opts, scalers)):
-            msg = clf.load_state_dict(checkpoint['classifiers'][k])
-            logger.info(f'loaded pretrained classifier {k} from epoch {epoch} with msg: {msg}')
-            opt.load_state_dict(checkpoint['opts'][k])
+            def part(key):
+                return checkpoint[key + 's'][k] if multihead else checkpoint[key]
+            msg = clf.load_state_dict(part('classifier'))
+            logger.info(f'loaded pretrained classifier{f" {k}" if multihead else ""} from epoch {epoch} with msg: {msg}')
+            opt.load_state_dict(part('opt'))
             if scaler is not None:
-                scaler.load_state_dict(checkpoint['scalers'][k])
-        logger.info(f'loaded optimizers of {len(classifiers)} heads from epoch {epoch}')
+                scaler.load_state_dict(part('scaler'))
+        logger.info(f'loaded optimizers{f" of {len(classifiers)} heads" if multihead else ""} from epoch {epoch}')
         logger.info(f'read-path: {r_path}')
         del checkpoint
     except Exception as e:
@@ -397,18 +370,48 @@ def load_clips(data, device, data_loader):
 def run_one_epoch(device, training, encoder, classifier, scaler, optimizer, scheduler, wd_scheduler, data_loader,
                   use_bfloat16, num_spatial_views, num_temporal_views, attend_across_segments, fp16_autocast=False):
     """eval.py:298-380.  Without attend_across_segments every (view, segment) token set goes through the classifier on
-    its own; the probe's backward adds all of them into one flat gradient buffer, exchanged once across ranks.
+    its own; the probe's backward adds all of them into one flat gradient buffer, exchanged once across ranks.  Loss and
+    scores are the reference's means of the cross-entropy and the softmax over views (and segments); see run_head_loop."""
+    def encode(data):
+        clips = load_clips(data, device, data_loader)
+        clip_indices = [d.to(device, non_blocking=True) for d in data[2]]
+        labels = data[1].to(device)
+        return encoder(clips, clip_indices), labels, len(labels)
 
-    classifier, scaler, optimizer, scheduler and wd_scheduler may also be lists, one entry per head
-    (optimization.multihead_kwargs): the encoder then runs once per batch, each head runs the loop body on its output in
-    turn (forward, loss, accuracy, backward, its own scaler and optimizer step), and the per-head accuracies are
-    returned.  One head computes what one classifier does."""
+    def loss_and_scores(outputs, labels):
+        if attend_across_segments:
+            loss = sum([F.cross_entropy(o, labels) for o in outputs]) / len(outputs)
+        else:
+            loss = (sum([sum([F.cross_entropy(ost, labels) for ost in os]) for os in outputs])
+                    / len(outputs) / len(outputs[0]))
+        with torch.no_grad():
+            if attend_across_segments:
+                scores = sum([F.softmax(o, dim=1) for o in outputs]) / len(outputs)
+            else:
+                scores = (sum([sum([F.softmax(ost, dim=1) for ost in os]) for os in outputs])
+                          / len(outputs) / len(outputs[0]))
+        return loss, scores
+
+    return run_head_loop(training, classifier, scaler, optimizer, scheduler, wd_scheduler, data_loader, use_bfloat16,
+                         fp16_autocast, encode, loss_and_scores)
+
+
+def run_head_loop(training, classifier, scaler, optimizer, scheduler, wd_scheduler, data_loader, use_bfloat16,
+                  fp16_autocast, encode, loss_and_scores):
+    """The batch loop of both drivers' run_one_epoch.  encode(data) -> (tokens, labels, batch size) runs once per batch
+    in the loop's autocast region under no_grad; then each head in turn calls its classifier on every tensor of the
+    (nested) token lists in that region, takes (loss, scores) from loss_and_scores(outputs, labels), scores top-1 by
+    the argmax of `scores` and steps its own scaler and optimizer.  classifier, scaler, optimizer, scheduler and
+    wd_scheduler are one of each (returns the accuracy) or per-head lists (returns the list of accuracies)."""
     multi = isinstance(classifier, (list, tuple))
     heads = list(zip(*[x if multi else [x] for x in (classifier, scaler, optimizer, scheduler, wd_scheduler)]))
     for clf, *_ in heads:
         clf.train(mode=training)
-    criterion = torch.nn.CrossEntropyLoss()
     top1_meters = [AverageMeter() for _ in heads]
+
+    def call(clf, tokens):
+        return [call(clf, t) for t in tokens] if isinstance(tokens, (list, tuple)) else clf(tokens)
+
     for itr, data in enumerate(data_loader):
 
         if training:
@@ -417,35 +420,17 @@ def run_one_epoch(device, training, encoder, classifier, scaler, optimizer, sche
                 wd_sched.step()
 
         # (without fp16_autocast no region: encoder and probe compute bf16 x bf16 -> fp32; see the module docstring)
-        with loop_autocast(fp16_autocast, use_bfloat16):
-            clips = load_clips(data, device, data_loader)
-            clip_indices = [d.to(device, non_blocking=True) for d in data[2]]
-            labels = data[1].to(device)
-            batch_size = len(labels)
-
-            with torch.no_grad():
-                tokens = encoder(clips, clip_indices)
+        with loop_autocast(fp16_autocast, use_bfloat16), torch.no_grad():
+            tokens, labels, batch_size = encode(data)
 
         for k, (clf, scaler, optimizer, _, _) in enumerate(heads):
             # the classifier calls run in the same region as the encoder; validation under no_grad
             with loop_autocast(fp16_autocast, use_bfloat16), torch.set_grad_enabled(training):
-                if attend_across_segments:
-                    outputs = [clf(o) for o in tokens]
-                else:
-                    outputs = [[clf(ost) for ost in os] for os in tokens]
+                outputs = call(clf, tokens)
 
-            if attend_across_segments:
-                loss = sum([criterion(o, labels) for o in outputs]) / len(outputs)
-            else:
-                loss = (sum([sum([criterion(ost, labels) for ost in os]) for os in outputs])
-                        / len(outputs) / len(outputs[0]))
+            loss, scores = loss_and_scores(outputs, labels)
             with torch.no_grad():
-                if attend_across_segments:
-                    outputs = sum([F.softmax(o, dim=1) for o in outputs]) / len(outputs)
-                else:
-                    outputs = (sum([sum([F.softmax(ost, dim=1) for ost in os]) for os in outputs])
-                               / len(outputs) / len(outputs[0]))
-                top1_acc = 100. * outputs.max(dim=1).indices.eq(labels).sum() / batch_size
+                top1_acc = 100. * scores.max(dim=1).indices.eq(labels).sum() / batch_size
                 top1_acc = float(AllReduce.apply(top1_acc))
                 top1_meters[k].update(top1_acc)
 
@@ -479,21 +464,7 @@ def step_head(classifier, scaler, optimizer, loss, use_bfloat16):
 
 def load_checkpoint(device, r_path, classifier, opt, scaler):
     """eval.py:383-411: classifier (module.-prefixed), optimizer and scaler state; any failure restarts at epoch 0."""
-    try:
-        checkpoint = torch.load(r_path, map_location=torch.device('cpu'))
-        epoch = checkpoint['epoch']
-        pretrained_dict = checkpoint['classifier']
-        msg = classifier.load_state_dict(pretrained_dict)
-        logger.info(f'loaded pretrained classifier from epoch {epoch} with msg: {msg}')
-        opt.load_state_dict(checkpoint['opt'])
-        if scaler is not None:
-            scaler.load_state_dict(checkpoint['scaler'])
-        logger.info(f'loaded optimizers from epoch {epoch}')
-        logger.info(f'read-path: {r_path}')
-        del checkpoint
-    except Exception as e:
-        logger.info(f'Encountered exception when loading checkpoint {e}')
-        epoch = 0
+    epoch = load_multihead_checkpoint(device, r_path, [classifier], [opt], [scaler], multihead_kwargs=None)
     return classifier, opt, scaler, epoch
 
 
