@@ -120,8 +120,10 @@ int vj_colsum(const void* in, int in_f32, float* out, long long T, int N, long l
 int vj_colsum_f16(const void* in, float* out, long long T, int N, long long ld, int period, int lo, int hi,
                   void* stream);
 
-/* Tubelet im2col: clips fp32 [B,C,T,H,W] -> patches bf16 [B*K', C*tub*ps*ps] in Conv3d weight order
- * (c,dt,dh,dw); idx (int64 [B,K], nullable) gathers tokens first (context path), else K' = all tokens.
+/* Tubelet im2col: clips fp32 [B,C,T,H,W] -> patches bf16 [B*K', P_pad] in Conv3d weight order (c,dt,dh,dw);
+ * idx (int64 [B,K], nullable) gathers tokens first (context path), else K' = all tokens.  P = C*tub*ps*ps, and each row
+ * is P_pad = round_up(P, 64) elements long (the GEMMs' N / lda granule): columns P..P_pad-1 are written as zeros
+ * (ps 14: P 1176 -> 1216 for video, 588 -> 640 for images; every ps-16 row is exactly P long).  ps must be even.
  * PatchEmbed3D, src/models/utils/patch_embed.py:47-57 (+ apply_masks, vision_transformer.py:178-180). */
 int vj_im2col_tubelets(const float* clips, void* patches, const long long* idx, int B, int C, int T, int H,
                        int W, int tubelet, int patch, int K, void* stream);
@@ -184,7 +186,7 @@ int vj_token_std_accum(const void* z, float* pstd, int B, int K, int D, float ep
 /* out bf16 [B*nq, H*HD] = softmax(q k^T * scale) v per (clip, head, query): CrossAttention.forward's SDPA
  * (src/models/utils/modules.py:138-153) for the nq learned query tokens of AttentivePooler
  * (src/models/attentive_pooler.py:96-102).  q bf16 [B*nq, H*HD]; kv bf16 [B*S, 2*H*HD] = the kv Linear's output
- * (k | v halves, head-major).  HD in {32, 64, 80, 128}. */
+ * (k | v halves, head-major).  HD in {32, 64, 80, 88, 104, 128}. */
 int vj_cross_attn_fwd(const void* q, const void* kv, void* out, int B, int nq, int S, int H, int HD, float scale,
                       void* stream);
 /* Same as vj_cross_attn_fwd (out bitwise identical), and also writes the softmax statistics lse2 fp32 [B*nq, H]
@@ -196,7 +198,7 @@ size_t vj_cross_attn_bwd_workspace(int B, int nq, int S, int H, int HD);
 /* Backward of the above (autograd of modules.py:138-153 for training the attentive probe).  From q, kv, out, dout
  * (bf16, layouts as in the forward) and lse2: dq fp32 [B*nq, H*HD], dkv bf16 [B*S, 2*H*HD] (dk | dv halves).
  * dk / dv sum over the clip's nq queries.  Deterministic: no atomics, every dkv element is written once and dq is
- * reduced over key chunks in a fixed order.  HD in {32, 64, 80, 128}. */
+ * reduced over key chunks in a fixed order.  HD in {32, 64, 80, 88, 104, 128}. */
 int vj_cross_attn_bwd(const void* q, const void* kv, const void* out, const void* dout, const float* lse2, float* dq,
                       void* dkv, void* workspace, size_t ws_bytes, int B, int nq, int S, int H, int HD, float scale,
                       void* stream);

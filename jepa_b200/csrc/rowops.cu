@@ -85,16 +85,19 @@ __global__ void __launch_bounds__(256) colsum_kernel(const void* __restrict__ in
 }
 
 // =============================================================================================
-// Tubelet im2col: clips fp32 [B,3,T,H,W] -> patches bf16 [rows, 3*tub*ps*ps], column order
+// Tubelet im2col: clips fp32 [B,3,T,H,W] -> patches bf16 [rows, ld], P = 3*tub*ps*ps, column order
 // (c, dt, dh, dw) = Conv3d weight flattening; row = (b, token) with token = (t', h', w') row-major
-// or the gathered token idx[b, k].  One warp per (row, c, dt) slab of ps*ps contiguous outputs.
+// or the gathered token idx[b, k].  One warp per (row, c, dt) slab of ps*ps contiguous outputs; V floats per load
+// (4 when ps % 4 == 0, else 2: ps 14 is 7 pairs per patch row).  PAD: rows are ld = round_up(P, 64) long and the warp
+// of the last slab also zeroes the ld - P pad columns; without PAD (P % 64 == 0, every ps-16 model) ld = P.
 // =============================================================================================
-template <typename TO>
+template <typename TO, int V, bool PAD>
 __global__ void __launch_bounds__(256) im2col_kernel(const float* __restrict__ clips, TO* __restrict__ out,
                                                      const long long* __restrict__ idx, int B, int C, int T, int H,
                                                      int W, int tub, int ps, int tokens_per_clip_out, int n_tokens) {
   const int gh = H / ps, gw = W / ps;
   const int P = C * tub * ps * ps;
+  const int ld = PAD ? (P + 63) / 64 * 64 : P;
   const int slabs = C * tub;  // slabs of ps*ps per row
   const long long total = (long long)B * tokens_per_clip_out * slabs;
   const int lane = threadIdx.x & 31;
@@ -110,15 +113,26 @@ __global__ void __launch_bounds__(256) im2col_kernel(const float* __restrict__ c
     const int c = slab / tub, dt = slab % tub;
     const int tw = int(tok % gw), th = int((tok / gw) % gh), tt = int(tok / ((long long)gw * gh));
     const float* src = clips + ((((long long)b * C + c) * T + (tt * tub + dt)) * H + (long long)th * ps) * W + tw * ps;
-    TO* dst = out + row * P + (long long)slab * ps * ps;
-    // ps*ps elements: dh rows of ps contiguous floats
-    for (int e = lane * 4; e < ps * ps; e += 128) {
+    TO* dst = out + row * ld + (long long)slab * ps * ps;
+    // ps*ps elements: dh rows of ps contiguous floats (ps % V == 0, so a load never crosses a row)
+    for (int e = lane * V; e < ps * ps; e += 32 * V) {
       const int dh = e / ps, dw = e % ps;
-      const float4 f = *reinterpret_cast<const float4*>(src + (long long)dh * W + dw);
-      uint2 o;
-      o.x = Elt<TO>::pack(f.x, f.y);
-      o.y = Elt<TO>::pack(f.z, f.w);
-      *reinterpret_cast<uint2*>(dst + e) = o;
+      if constexpr (V == 4) {
+        const float4 f = *reinterpret_cast<const float4*>(src + (long long)dh * W + dw);
+        uint2 o;
+        o.x = Elt<TO>::pack(f.x, f.y);
+        o.y = Elt<TO>::pack(f.z, f.w);
+        *reinterpret_cast<uint2*>(dst + e) = o;
+      } else {
+        const float2 f = *reinterpret_cast<const float2*>(src + (long long)dh * W + dw);
+        *reinterpret_cast<uint32_t*>(dst + e) = Elt<TO>::pack(f.x, f.y);
+      }
+    }
+    if constexpr (PAD) {
+      if (slab == slabs - 1) {
+        TO* const pad = dst - (long long)slab * ps * ps + P;
+        for (int e = lane * 2; e < ld - P; e += 64) *reinterpret_cast<uint32_t*>(pad + e) = 0u;
+      }
     }
   }
 }
@@ -517,14 +531,24 @@ template <typename TO>
 static int im2col_tubelets(const float* clips, void* patches, const long long* idx, int B, int C, int T, int H, int W,
                            int tubelet, int patch, int K, cudaStream_t s) {
   VJ_CHECK_ARG(clips && patches, "vj_im2col_tubelets: null pointer");
-  VJ_CHECK_ARG(T % tubelet == 0 && H % patch == 0 && W % patch == 0 && patch % 4 == 0 && W % 4 == 0,
-               "vj_im2col_tubelets: bad geometry");
+  // W % patch == 0 and an even patch keep every 8-byte (ps % 4 != 0) or 16-byte (ps % 4 == 0) load aligned
+  VJ_CHECK_ARG(T % tubelet == 0 && H % patch == 0 && W % patch == 0 && patch % 2 == 0,
+               "vj_im2col_tubelets: bad geometry (T %% tubelet, H %% patch, W %% patch must be 0 and patch even)");
   const int n_tokens = (T / tubelet) * (H / patch) * (W / patch);
   const int kout = idx ? K : n_tokens;
   if (B <= 0 || kout <= 0) return 0;
+  const int P = C * tubelet * patch * patch;
   const long long warps = (long long)B * kout * C * tubelet;
-  im2col_kernel<TO><<<grid_for(warps, 8), 256, 0, s>>>(clips, reinterpret_cast<TO*>(patches), idx, B, C, T, H, W,
-                                                       tubelet, patch, kout, n_tokens);
+  TO* out = reinterpret_cast<TO*>(patches);
+  if (patch % 4 == 0 && P % 64 == 0)   // every ps-16 model: rows exactly P long
+    im2col_kernel<TO, 4, false><<<grid_for(warps, 8), 256, 0, s>>>(clips, out, idx, B, C, T, H, W, tubelet, patch, kout,
+                                                                   n_tokens);
+  else if (patch % 4 == 0)
+    im2col_kernel<TO, 4, true><<<grid_for(warps, 8), 256, 0, s>>>(clips, out, idx, B, C, T, H, W, tubelet, patch, kout,
+                                                                  n_tokens);
+  else
+    im2col_kernel<TO, 2, true><<<grid_for(warps, 8), 256, 0, s>>>(clips, out, idx, B, C, T, H, W, tubelet, patch, kout,
+                                                                  n_tokens);
   VJ_CUDA(cudaGetLastError());
   vj::count_launch(1);
   return 0;

@@ -115,7 +115,8 @@ __global__ void __launch_bounds__(kXattnThreads) xattn_fwd_kernel(const T* __res
 }
 
 // sum over the LPK lanes of a key's lane group; every lane of the group gets the same value (butterfly when LPK is a
-// power of two, rotation otherwise - hd 80 has 10 lanes per key)
+// power of two, rotation otherwise - hd 80 / 88 / 104 have 10 / 11 / 13 lanes per key).  Lanes past the last whole
+// group (32 % LPK of them) hold no key; their shuffles may read another group's lanes and their sums are never used.
 template <int LPK>
 VJ_DEVINL float group_sum(float v) {
   if constexpr ((LPK & (LPK - 1)) == 0) {
@@ -265,6 +266,8 @@ static int xattn_bwd_chunks(int S, int HD) {
     case 32: kpc = xattn_bwd_chunk<4>(); break;
     case 64: kpc = xattn_bwd_chunk<8>(); break;
     case 80: kpc = xattn_bwd_chunk<10>(); break;
+    case 88: kpc = xattn_bwd_chunk<11>(); break;
+    case 104: kpc = xattn_bwd_chunk<13>(); break;
     case 128: kpc = xattn_bwd_chunk<16>(); break;
     default: return -1;
   }
@@ -292,8 +295,10 @@ static int cross_attn_fwd(const char* name, const void* q, const void* kv, void*
     case 32: VJ_XATTN(4); break;
     case 64: VJ_XATTN(8); break;
     case 80: VJ_XATTN(10); break;
+    case 88: VJ_XATTN(11); break;
+    case 104: VJ_XATTN(13); break;
     case 128: VJ_XATTN(16); break;
-    default: set_error("%s: head dim %d unsupported (32 / 64 / 80 / 128)", name, HD); return -1;
+    default: set_error("%s: head dim %d unsupported (32 / 64 / 80 / 88 / 104 / 128)", name, HD); return -1;
   }
 #undef VJ_XATTN
   VJ_CUDA(cudaGetLastError());
@@ -337,7 +342,7 @@ static int cross_attn_bwd(const char* name, const void* q, const void* kv, const
   VJ_CHECK_ARG(q && kv && out && dout && lse2 && dq && dkv && workspace, "%s: null pointer", name);
   VJ_CHECK_ARG(B > 0 && nq > 0 && S > 0 && H > 0, "%s: empty problem", name);
   const int nchunk = xattn_bwd_chunks(S, HD);
-  VJ_CHECK_ARG(nchunk > 0, "%s: head dim %d unsupported (32 / 64 / 80 / 128)", name, HD);
+  VJ_CHECK_ARG(nchunk > 0, "%s: head dim %d unsupported (32 / 64 / 80 / 88 / 104 / 128)", name, HD);
   VJ_CHECK_ARG(nchunk <= 65535, "%s: S = %d keys is too long", name, S);
   VJ_CHECK_ARG(ws_bytes >= vj_cross_attn_bwd_workspace(B, nq, S, H, HD), "%s: workspace too small", name);
   VJ_CHECK_ARG(((reinterpret_cast<uintptr_t>(q) | reinterpret_cast<uintptr_t>(kv) | reinterpret_cast<uintptr_t>(out) |
@@ -354,6 +359,8 @@ static int cross_attn_bwd(const char* name, const void* q, const void* kv, const
     case 32: VJ_XATTN_BWD(4); break;
     case 64: VJ_XATTN_BWD(8); break;
     case 80: VJ_XATTN_BWD(10); break;
+    case 88: VJ_XATTN_BWD(11); break;
+    case 104: VJ_XATTN_BWD(13); break;
     case 128: VJ_XATTN_BWD(16); break;
   }
 #undef VJ_XATTN_BWD

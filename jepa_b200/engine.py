@@ -15,7 +15,7 @@ import math
 import torch
 
 from . import kernels as K
-from .params import padded_head_dim
+from .params import padded_head_dim, padded_patch_dim
 
 BF16, F16, F32 = torch.bfloat16, torch.float16, torch.float32
 LN_EPS = 1e-6  # norm_layer=partial(nn.LayerNorm, eps=1e-6): vision_transformer.py:252, predictor.py:244
@@ -268,6 +268,23 @@ class _LayerTaps:
             self.outs.append(y)
 
 
+def patch_embed_weight(mod, store, dtype):
+    """[D, P_pad] `dtype` operand of the patch-embedding GEMM (P_pad = padded_patch_dim(P), the im2col row length): the
+    shadow itself when P is a multiple of 64, else a copy zero-padded from the fp32 master (zero columns meet the zero
+    pad columns of the patches, so the products are unchanged)."""
+    D = mod.embed_dim
+    P = mod.patch_embed.proj.weight[0].numel()
+    Pp = padded_patch_dim(P)
+    if Pp == P:
+        return store.w16("patch_embed.proj.weight", dtype).view(D, P)
+    key = ("pad_pe", dtype)
+    buf = mod._scratch.get(key)
+    if buf is None:
+        buf = mod._scratch[key] = _empty((D, Pp), dtype, store.flat.device)
+    K.head_pad(store.f32("patch_embed.proj.weight").view(D, P), buf, D, 1, P, Pp, 1)
+    return buf
+
+
 def pos_interp_scales(grid0, grid, video):
     """scale_factor that interpolate_pos_encoding (vision_transformer.py:197-246) hands to F.interpolate to take the
     table of token grid `grid0` to `grid`: (T'/Nt, H'/Nh, W'/Nw) for video, sqrt(npatch / N) on both axes for images."""
@@ -314,8 +331,9 @@ def encoder_forward(mod, clips, masks, save, final_norm=True, out_layers=None, g
     B = clips.shape[0]
     grid = mod.grid if grid is None else tuple(grid)
     N, D = grid[0] * grid[1] * grid[2], mod.embed_dim
-    P = mod.patch_embed.proj.weight[0].numel()
+    Pp = padded_patch_dim(mod.patch_embed.proj.weight[0].numel())     # im2col row length
     weights = gather_block_weights(store, spec, mod._scratch, dt)
+    w_pe = patch_embed_weight(mod, store, dt)
     clips = clips.contiguous()
     if clips.dtype != F32:
         clips = clips.float()
@@ -323,7 +341,7 @@ def encoder_forward(mod, clips, masks, save, final_norm=True, out_layers=None, g
         segments = [(B, N)]
         seq = cu_seqlens_for(segments, dev)
         T = seq[3]
-        patches = _empty((T, P), dt, dev)
+        patches = _empty((T, Pp), dt, dev)
         K.im2col_tubelets(clips, patches, None, mod.tubelet_size, mod.patch_size)
         rowmap, period = None, N
     else:
@@ -331,7 +349,7 @@ def encoder_forward(mod, clips, masks, save, final_norm=True, out_layers=None, g
         segments = [(B, int(m.shape[1])) for m in masks]
         seq = cu_seqlens_for(segments, dev)
         T = seq[3]
-        patches = _empty((T, P), dt, dev)
+        patches = _empty((T, Pp), dt, dev)
         off = 0
         for m in masks:
             n = B * m.shape[1]
@@ -340,7 +358,6 @@ def encoder_forward(mod, clips, masks, save, final_norm=True, out_layers=None, g
         rowmap = torch.cat([m.reshape(-1) for m in masks]).to(torch.int32)
         period = 0
     x = _empty((T, D), dt, dev)
-    w_pe = store.w16("patch_embed.proj.weight", dt).view(D, P)
     pos = encoder_pos(mod, store, grid, dev)
     K.gemm(patches, w_pe, x, bias=store.f32("patch_embed.proj.bias"), epi=K.EPI_ADD, aux=pos, aux_rowmap=rowmap,
            aux_period=period)
@@ -379,8 +396,17 @@ def encoder_backward(mod, sv, dout):
                     gv("norm.weight"), gv("norm.bias"))
     sync = _sync_begin(mod, gflat)
     dx = blocks_backward(spec, sv.weights, sv.blocks, dx, sv.seq, store, gflat, mod._scratch, sync)
-    P = sv.patches.shape[1]
-    _wgrad(dx, sv.patches, gv("patch_embed.proj.weight").view(D, P), gv("patch_embed.proj.bias"), T)
+    P, Pp = mod.patch_embed.proj.weight[0].numel(), sv.patches.shape[1]
+    gw = gv("patch_embed.proj.weight").view(D, P)
+    if Pp == P:
+        _wgrad(dx, sv.patches, gw, gv("patch_embed.proj.bias"), T)
+    else:   # N = P_pad into fp32 scratch, then its first P columns into the flat buffer; the pad columns are dropped
+        pg = mod._scratch.get("pad_pe_grad")
+        if pg is None:
+            pg = mod._scratch["pad_pe_grad"] = _empty((D, Pp), F32, dev)
+        pg.zero_()
+        _wgrad(dx, sv.patches, pg, gv("patch_embed.proj.bias"), T)
+        K.head_pad(pg, gw, D, 1, P, Pp, 1, unpad_add=True)
     if sync is not None:
         sync.finish()
     return gflat

@@ -169,7 +169,8 @@ def colsum(x, out, period=0, lo=0, hi=0):
 
 
 def im2col_tubelets(clips, patches, idx, tubelet, patch):
-    """patches bf16, or fp16."""
+    """patches bf16 or fp16 [B*K', padded_patch_dim(C*tubelet*patch*patch)] (pad columns written as zeros)."""
+    from .params import padded_patch_dim
     name = _f16("vj_im2col_tubelets", patches)
     _chk(clips, F32, "clips"); _chk(patches, None, "patches")
     B, C, T, H, W = clips.shape
@@ -177,6 +178,10 @@ def im2col_tubelets(clips, patches, idx, tubelet, patch):
     if idx is not None:
         _chk(idx, torch.int64, "idx")
         K = idx.shape[1]
+    rows = B * (K if idx is not None else (T // tubelet) * (H // patch) * (W // patch))
+    want = (rows, padded_patch_dim(C * tubelet * patch * patch))
+    if patches.dim() != 2 or tuple(patches.shape) != want:
+        raise _lib.VJError(f"im2col_tubelets: patches must be {want}, got {tuple(patches.shape)}")
     _lib.call(name, _p(clips), _p(patches), _p(idx), B, C, T, H, W, tubelet, patch, K, _s())
     return patches
 

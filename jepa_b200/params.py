@@ -28,6 +28,13 @@ def padded_head_dim(hd):
     raise ValueError(f"head dim {hd} > 128 is not supported by the attention kernels")
 
 
+def padded_patch_dim(p):
+    """Row length of the patch matrix vj_im2col_tubelets writes for patch vectors of length p: p rounded up to the GEMMs'
+    64-element granule (the weight gradient's N, TMA-aligned rows).  ps 16: 1536 / 768 unchanged; ps 14: 1176 -> 1216
+    (video), 588 -> 640 (images)."""
+    return (p + 63) // 64 * 64
+
+
 class FlatParamStore:
     def __init__(self):
         self.flat = None      # fp32 [total]

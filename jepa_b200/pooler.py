@@ -102,8 +102,9 @@ class AttentivePooler(nn.Module):
         if depth != 1:
             raise NotImplementedError("AttentivePooler depth > 1 (extra self-attention blocks over the query tokens) is not "
                                       "used by the frozen evaluations (eval.py:182-187 builds depth=1)")
-        if embed_dim % num_heads or (embed_dim // num_heads) not in (32, 64, 80, 128):
-            raise NotImplementedError(f"head dim {embed_dim // num_heads}: vj_cross_attn_fwd supports 32 / 64 / 80 / 128")
+        if embed_dim % num_heads or (embed_dim // num_heads) not in (32, 64, 80, 88, 104, 128):
+            raise NotImplementedError(f"head dim {embed_dim // num_heads}: vj_cross_attn_fwd supports 32 / 64 / 80 / 88 / "
+                                      "104 / 128")
         self.query_tokens = nn.Parameter(torch.zeros(1, num_queries, embed_dim))
         self.complete_block = complete_block
         if complete_block:

@@ -515,7 +515,7 @@ def run_xattn(args):
     g = torch.Generator(device="cpu").manual_seed(0)
     ev = [torch.cuda.Event(enable_timing=True) for _ in range(3)]
     rows = []
-    for hd in (64, 80):
+    for hd in args.head_dims:
         D = H * hd
         ref = {"q": torch.randn(B * nq, D, generator=g), "kv": torch.randn(B * S, 2 * D, generator=g),
                "dout": torch.randn(B * nq, D, generator=g)}
@@ -551,7 +551,8 @@ def run_xattn(args):
     card = _card()
     print(json.dumps({
         "metric": "cross-attention forward (with lse) and backward, bf16 vs fp16, K400 probe shape",
-        "config": {"workload": f"B {B}, S {S}, H {H}, nq {nq}, hd 64 (ViT-L) and 80 (ViT-H)"},
+        "config": {"workload": f"B {B}, S {S}, H {H}, nq {nq}, hd {', '.join(map(str, args.head_dims))} "
+                               "(ViT-L 64, ViT-H 80, ViT-g 88, ViT-G 104)"},
         "rows": rows,
         "timing": "CUDA events around each launch (backward: both kernels), median over the timed repetitions, the two "
                   "dtypes alternating; GB/s from the kv read (forward) and the kv read + dkv write (backward)",
@@ -577,7 +578,10 @@ def main():
                     help="train / val / image mode: comma-separated probe counts trained (validated) on one encoder "
                          "pass, e.g. 1,4,16, alternated step by step; reports encoder ms, probe ms per head and "
                          "throughput for each")
+    ap.add_argument("--head-dims", default="64,80",
+                    help="xattn mode: comma-separated head dims timed, e.g. 80,88,104,128")
     args = ap.parse_args()
+    args.head_dims = [int(h) for h in args.head_dims.split(",")]
     args.multi = args.heads is not None
     args.heads = [int(n) for n in args.heads.split(",")] if args.multi else [1]
     if any(n < 1 for n in args.heads) or len(set(args.heads)) != len(args.heads):
