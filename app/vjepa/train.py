@@ -7,6 +7,12 @@ Same config schema, schedules, CSV columns, log lines and checkpoint format as t
   L1 latent loss / variance reg -> jepa_b200.step.jepa_loss/reg_loss  (train.py:440-459)
   AdamW                         -> jepa_b200.optim.FlatAdamW          (train.py:462-475)
   EMA                           -> jepa_b200.step.ema_update          (train.py:484-487)
+
+`optimization.accum_iter: k` (default 1; the reference has no such key) accumulates k loader batches of
+`data.batch_size` clips into each optimizer step, so a recipe's global batch is reachable on fewer GPUs: the first
+k - 1 backwards run under DistributedDataParallel.no_sync() and add into the flat gradient buffers, the last one adds
+and all-reduces.  `ipe` counts optimizer steps (an epoch reads ipe * k loader batches), so the LR / WD / EMA schedules
+mean what they mean at k = 1; one CSV row per optimizer step, its losses the mean over the k micro-batches.
 """
 import os
 
@@ -16,6 +22,7 @@ try:
 except Exception:
     pass
 
+import contextlib
 import copy
 import time
 
@@ -123,6 +130,9 @@ def main(args, resume_preempt=False):
     ema = opt_cfg.get('ema')
     betas = opt_cfg.get('betas', (0.9, 0.999))
     eps = opt_cfg.get('eps', 1.e-8)
+    accum_iter = opt_cfg.get('accum_iter', 1)      # loader batches (micro-batches) per optimizer step
+    if isinstance(accum_iter, bool) or not isinstance(accum_iter, int) or accum_iter < 1:
+        raise ValueError(f"optimization.accum_iter must be an integer >= 1, got {accum_iter!r}")
 
     log_cfg = args.get('logging')
     folder = log_cfg.get('folder')
@@ -177,13 +187,15 @@ def main(args, resume_preempt=False):
         frame_sample_rate=sampling_rate, filter_short_videos=filter_short_videos, decode_one_clip=decode_one_clip,
         duration=duration, num_clips=num_clips, transform=transform, datasets_weights=datasets_weights,
         collator=mask_collator, num_workers=num_workers, world_size=world_size, pin_mem=pin_mem, rank=rank,
-        log_dir=folder if log_resource_util_data else None, crop_size=crop_size, ipe=ipe or 300)
+        log_dir=folder if log_resource_util_data else None, crop_size=crop_size, ipe=(ipe or 300) * accum_iter)
     try:
         _dlen = len(unsupervised_loader)
     except Exception:
         _dlen = unsupervised_loader.num_batches
     if ipe is None:
-        ipe = _dlen
+        ipe = _dlen // accum_iter
+        if ipe < 1:
+            raise ValueError(f"optimization.accum_iter={accum_iter} exceeds the {_dlen} batches of the loader")
     logger.info(f'iterations per epoch/dataest length: {ipe}/{_dlen}')
 
     optimizer, scaler, scheduler, wd_scheduler = init_opt(
@@ -208,7 +220,8 @@ def main(args, resume_preempt=False):
             scheduler.step()
             wd_scheduler.step()
             next(momentum_scheduler)
-            mask_collator.step()
+            for _ in range(accum_iter):     # the collator drew masks for every loader batch of those steps
+                mask_collator.step()
 
     checkpointer = AsyncCheckpointer()
 
@@ -220,6 +233,8 @@ def main(args, resume_preempt=False):
             'scaler': None if scaler is None else scaler.state_dict(), 'target_encoder': target_encoder.state_dict(),
             'epoch': epoch, 'loss': loss_meter.avg, 'batch_size': batch_size, 'world_size': world_size, 'lr': lr,
         }
+        if accum_iter > 1:      # batch_size stays the per-GPU micro-batch; the global batch is their product
+            save_dict['accum_iter'] = accum_iter
         # asynchronous: device->host snapshot enqueued now, serialisation + disk write in a background thread
         checkpointer.save(save_dict, path)
         if checkpointer.error is not None:
@@ -257,42 +272,56 @@ def main(args, resume_preempt=False):
 
         for itr in range(ipe):
             itr_start_time = time.time()
-            try:
-                udata, masks_enc, masks_pred = next(loader)
-            except Exception:
-                logger.info('Exhausted data loaders. Refreshing...')
-                loader = iter(unsupervised_loader)
-                udata, masks_enc, masks_pred = next(loader)
-            assert len(masks_enc) == len(masks_pred), 'Currently require num encoder masks = num predictor masks'
+            micro = []      # (clips, masks_enc, masks_pred) of each of the accum_iter loader batches of this step
+            for _ in range(accum_iter):
+                try:
+                    udata, masks_enc, masks_pred = next(loader)
+                except Exception:
+                    logger.info('Exhausted data loaders. Refreshing...')
+                    loader = iter(unsupervised_loader)
+                    udata, masks_enc, masks_pred = next(loader)
+                assert len(masks_enc) == len(masks_pred), 'Currently require num encoder masks = num predictor masks'
 
-            # host -> device; every clip of a sample reuses that sample's mask pair (train.py:391-409)
-            def to_device(u):
-                if isinstance(u, (list, tuple)):   # tickets: uint8 frames cross PCIe, the kernels augment / crop / normalise
-                    return tickets_to_device(list(u), device, crop_size)
-                return u.to(device, non_blocking=True)
-            clips = torch.cat([to_device(u) for u in udata[0]], dim=0)
-            masks_enc = [repeat_interleave_batch(m.to(device, non_blocking=True), batch_size, repeat=num_clips)
-                         for m in masks_enc]
-            masks_pred = [repeat_interleave_batch(m.to(device, non_blocking=True), batch_size, repeat=num_clips)
-                          for m in masks_pred]
-            for _i, m in enumerate(mask_meters):
-                m.update(masks_enc[_i][0].size(-1))
+                # host -> device; every clip of a sample reuses that sample's mask pair (train.py:391-409)
+                def to_device(u):
+                    if isinstance(u, (list, tuple)):   # tickets: uint8 frames cross PCIe, the kernels augment / crop / normalise
+                        return tickets_to_device(list(u), device, crop_size)
+                    return u.to(device, non_blocking=True)
+                clips = torch.cat([to_device(u) for u in udata[0]], dim=0)
+                masks_enc = [repeat_interleave_batch(m.to(device, non_blocking=True), batch_size, repeat=num_clips)
+                             for m in masks_enc]
+                masks_pred = [repeat_interleave_batch(m.to(device, non_blocking=True), batch_size, repeat=num_clips)
+                              for m in masks_pred]
+                for _i, m in enumerate(mask_meters):
+                    m.update(masks_enc[_i][0].size(-1))
+                micro.append((clips, masks_enc, masks_pred))
 
             def train_step():
                 _new_lr = scheduler.step()
                 _new_wd = wd_scheduler.step()
 
-                # Step 1. forward (bf16 tensor-core math, fp32 accumulation - the reference's autocast region)
-                h = vj.forward_target(target_encoder, clips, masks_pred)
-                z = encoder(clips, masks_enc)
-                z = predictor(z, h, masks_enc, masks_pred)
-                loss_jepa = vj.jepa_loss(z, h, loss_exp)
-                loss_reg = vj.reg_loss(z, with_grad=(reg_coeff != 0.0))   # differentiable only when it is used
-                loss = loss_jepa + reg_coeff * loss_reg
+                losses = []
+                for i, (clips, masks_enc, masks_pred) in enumerate(micro):
+                    with contextlib.ExitStack() as no_sync:
+                        if i < accum_iter - 1:      # add into the gradient buffers; the last backward exchanges the sum
+                            no_sync.enter_context(encoder.no_sync())
+                            no_sync.enter_context(predictor.no_sync())
+                        # Step 1. forward (bf16 tensor-core math, fp32 accumulation - the reference's autocast region);
+                        # every micro-batch of the step sees the same target weights
+                        h = vj.forward_target(target_encoder, clips, masks_pred)
+                        z = encoder(clips, masks_enc)
+                        z = predictor(z, h, masks_enc, masks_pred)
+                        loss_jepa = vj.jepa_loss(z, h, loss_exp)
+                        loss_reg = vj.reg_loss(z, with_grad=(reg_coeff != 0.0))   # differentiable only when it is used
+                        loss = loss_jepa + reg_coeff * loss_reg
 
-                # Step 2. backward & optimizer step (GradScaler kept: it is active for bf16 in the reference too)
+                        # Step 2. backward (GradScaler kept: it is active for bf16 in the reference too); the
+                        # accumulated gradient is the mean over the micro-batches, as over one batch of k times the size
+                        scaler.scale(loss if accum_iter == 1 else loss / accum_iter).backward()
+                    losses.append((loss, loss_jepa, loss_reg))
+
+                # optimizer step, once per accum_iter micro-batches: an inf / NaN in any of them skips the whole step
                 _enc_norm, _pred_norm = 0., 0.
-                scaler.scale(loss).backward()
                 scaler.unscale_(optimizer)
                 if (epoch > warmup) and (clip_grad is not None):
                     _enc_norm = vj.clip_grad_norm_(encoder, clip_grad)
@@ -309,18 +338,19 @@ def main(args, resume_preempt=False):
                 # Step 3. momentum update of the target encoder
                 vj.ema_update(encoder, target_encoder, next(momentum_scheduler))
 
-                return (float(loss), float(loss_jepa), float(loss_reg), _new_lr, _new_wd, grad_stats, grad_stats_pred,
-                        optim_stats)
+                loss, loss_jepa, loss_reg = (sum(float(l[j]) for l in losses) / accum_iter for j in range(3))
+                return loss, loss_jepa, loss_reg, _new_lr, _new_wd, grad_stats, grad_stats_pred, optim_stats
 
             (loss, loss_jepa, loss_reg, _new_lr, _new_wd, grad_stats, grad_stats_pred, optim_stats), gpu_etime_ms = \
                 gpu_timer(train_step)
             iter_elapsed_time_ms = (time.time() - itr_start_time) * 1000.
             loss_meter.update(loss)
-            flat_clips = clips.view(clips.shape[0], -1)
-            input_var = float(AllReduce.apply(flat_clips.var(dim=1).mean(dim=0)))
-            input_var_min = float(AllReduce.apply(torch.min(flat_clips.var(dim=1))))
-            input_var_meter.update(input_var)
-            input_var_min_meter.update(input_var_min)
+            for clips, _, _ in micro:
+                flat_clips = clips.view(clips.shape[0], -1)
+                input_var = float(AllReduce.apply(flat_clips.var(dim=1).mean(dim=0)))
+                input_var_min = float(AllReduce.apply(torch.min(flat_clips.var(dim=1))))
+                input_var_meter.update(input_var)
+                input_var_min_meter.update(input_var_min)
             jepa_loss_meter.update(loss_jepa)
             reg_loss_meter.update(loss_reg)
             gpu_time_meter.update(gpu_etime_ms)

@@ -5,6 +5,7 @@ behaviour (early return if a group exists, SLURM variables, port 37123, fall bac
 failure); the backend is NCCL when CUDA is present and gloo otherwise so the host logic can be
 exercised on CPU-only machines.
 """
+import contextlib
 import os
 from logging import getLogger
 
@@ -154,6 +155,7 @@ class FlatGradSync:
         self.hi = 0         # everything in [hi, total) has been handed to NCCL already
         self.lo = 0         # everything in [lo, hi) is final but not yet sent
         self.n_calls = 0    # all-reduces issued for the current buffer (tests / launch accounting)
+        self.paused = 0     # > 0 inside DistributedDataParallel.no_sync(): backwards accumulate locally
 
     def begin(self, gflat):
         # a backward that raised after queueing its end-of-backward callback would leave the flag set and make every
@@ -213,11 +215,15 @@ class ProbeGradSync:
         self.group = process_group
         self.gflat = None
         self.n_calls = 0    # all-reduces issued (tests)
+        self.paused = 0     # > 0 inside DistributedDataParallel.no_sync(): backwards accumulate locally
 
     def mark(self, gflat):
         """Called by every probe backward with the buffer it accumulated into.  Each call queues an end-of-backward
         callback; the first one to run exchanges the buffer and the others find nothing left to do, so a pass issues
-        exactly one all-reduce (and a backward that raised part-way leaves nothing armed for the next one)."""
+        exactly one all-reduce (and a backward that raised part-way leaves nothing armed for the next one).  Inside
+        no_sync() nothing is queued: the buffer keeps accumulating until the first backward outside it."""
+        if self.paused:
+            return
         self.gflat = gflat
         torch.autograd.Variable._execution_engine.queue_callback(self._exchange)
 
@@ -260,8 +266,24 @@ class DistributedDataParallel(torch.nn.Module):
     def forward(self, *args, **kwargs):
         return self.module(*args, **kwargs)
 
+    @contextlib.contextmanager
     def no_sync(self):
-        """torch DDP's gradient-accumulation context is NOT supported: every backward writes a fresh flat gradient buffer
-        and all-reduces it in place while the backward is still running, so a second backward before zero_grad() would
-        accumulate into partially reduced data.  The reference never accumulates (app/vjepa/train.py:462-483)."""
-        raise NotImplementedError("jepa_b200 DistributedDataParallel: gradient accumulation / no_sync() is not supported")
+        """torch DDP's gradient-accumulation context.  A backward run inside it adds into the flat gradient buffer its
+        .grads already are (or starts one) and exchanges nothing: no all-reduce, no end-of-backward callback, no SM
+        reservation.  The first backward outside it adds its own gradients and then all-reduces the accumulated buffer
+        with the usual bucketed, in-place averaging exchange; that backward still writes the buffer from its end towards
+        its start, so the buckets become final in the same order as without accumulation.  Contexts nest, and leaving
+        one (also by an exception) leaves nothing armed.  Like torch DDP, every rank must run the same number of
+        backwards inside and outside the context, or the collectives stop matching."""
+        syncs = {}
+        for m in self.module.modules():
+            for s in (getattr(m, "_vj_grad_sync", None), getattr(m, "_vj_probe_sync", None)):
+                if s is not None:
+                    syncs[id(s)] = s
+        for s in syncs.values():
+            s.paused += 1
+        try:
+            yield
+        finally:
+            for s in syncs.values():
+                s.paused -= 1

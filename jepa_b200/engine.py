@@ -182,10 +182,12 @@ def _wgrad(dy, act, grad_out, bias_grad, tokens):
 
 
 def _sync_begin(mod, gflat):
-    """Data-parallel gradient exchange (jepa_b200.distributed.FlatGradSync) attached to this network, or None."""
+    """Data-parallel gradient exchange (jepa_b200.distributed.FlatGradSync) attached to this network, or None (also
+    inside DistributedDataParallel.no_sync(), where the backward only accumulates)."""
     sync = getattr(mod, "_vj_grad_sync", None)
-    if sync is not None:
-        sync.begin(gflat)
+    if sync is None or sync.paused:
+        return None
+    sync.begin(gflat)
     return sync
 
 
@@ -383,11 +385,13 @@ def encoder_forward(mod, clips, masks, save, final_norm=True, out_layers=None, g
     return out, sv, segments
 
 
-def encoder_backward(mod, sv, dout):
-    """dout bf16 [T, D] = grad wrt the normalised encoder output.  Returns the flat fp32 grad buffer."""
+def encoder_backward(mod, sv, dout, gflat=None):
+    """dout bf16 [T, D] = grad wrt the normalised encoder output.  Returns the flat fp32 grad buffer: `gflat` when given
+    (every gradient producer below adds into the buffer, so this accumulates onto what it holds), else a new one."""
     store = sv.store
     spec = mod._spec
-    gflat = store.new_grad_buffer()
+    if gflat is None:
+        gflat = store.new_grad_buffer()
     gv = lambda name: store.grad_view(gflat, name)
     T, D = dout.shape
     dev = dout.device
@@ -484,8 +488,9 @@ def predictor_forward(mod, z_cat, masks_ctxt, masks_tgt, mask_indices, save):
     return out, sv
 
 
-def predictor_backward(mod, sv, dout):
-    """dout bf16 [sum B*Kp_i, D_enc].  Returns (dz_cat bf16 [sum B*Ke_i, D_enc], flat grad buffer)."""
+def predictor_backward(mod, sv, dout, gflat=None):
+    """dout bf16 [sum B*Kp_i, D_enc].  Returns (dz_cat bf16 [sum B*Ke_i, D_enc], flat grad buffer): `gflat`, added into,
+    when given, else a new one."""
     store = sv.store
     spec = mod._spec
     dev = dout.device
@@ -493,7 +498,8 @@ def predictor_backward(mod, sv, dout):
     B, Ke, Kp = sv.B, sv.Ke, sv.Kp
     T = sv.seq[3]
     Tt, Denc = dout.shape
-    gflat = store.new_grad_buffer()
+    if gflat is None:
+        gflat = store.new_grad_buffer()
     gv = lambda name: store.grad_view(gflat, name)
     dout = dout.contiguous()
     # predictor_proj

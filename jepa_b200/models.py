@@ -123,6 +123,20 @@ def _common_base(tensors):
 # -------------------------------------------------------------------------------------------------
 # autograd glue
 # -------------------------------------------------------------------------------------------------
+def _live_grad_buffer(mod, store):
+    """The flat buffer the .grads of every trainable parameter of `mod` already alias (a backward since zero_grad(): the
+    earlier micro-batches of gradient accumulation), or None."""
+    return store.live_grad_buffer(p for p in mod.parameters() if p.requires_grad)
+
+
+def _param_grads(mod, store, gflat, live):
+    """What the backward hands autograd for mod's parameters: views of the new buffer `gflat` (AccumulateGrad makes them
+    the .grads), or nothing when the backward added into the live buffer the .grads already are."""
+    if live is not None:
+        return [None] * len(list(mod.parameters()))
+    return [store.grad_view(gflat, n) if p.requires_grad else None for n, p in mod.named_parameters()]
+
+
 class _EncoderFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, mod, clips, masks, final_norm, grid, grad_enabled, *params):
@@ -137,10 +151,10 @@ class _EncoderFn(torch.autograd.Function):
     @staticmethod
     def backward(ctx, dout):
         mod, sv = ctx.mod, ctx.sv
-        gflat = engine.encoder_backward(mod, sv, dout)
+        live = _live_grad_buffer(mod, sv.store)
+        gflat = engine.encoder_backward(mod, sv, dout, live)
         ctx.sv = None
-        grads = [sv.store.grad_view(gflat, n) if p.requires_grad else None for n, p in mod.named_parameters()]
-        return (None, None, None, None, None, None, *grads)
+        return (None, None, None, None, None, None, *_param_grads(mod, sv.store, gflat, live))
 
 
 class _PredictorFn(torch.autograd.Function):
@@ -154,10 +168,11 @@ class _PredictorFn(torch.autograd.Function):
     @staticmethod
     def backward(ctx, dout):
         mod, sv = ctx.mod, ctx.sv
-        dz, gflat = engine.predictor_backward(mod, sv, dout)
+        live = _live_grad_buffer(mod, sv.store)
+        dz, gflat = engine.predictor_backward(mod, sv, dout, live)
         ctx.sv = None
-        grads = [sv.store.grad_view(gflat, n) if p.requires_grad else None for n, p in mod.named_parameters()]
-        return (None, dz if ctx.needs_input_grad[1] else None, None, None, None, *grads)
+        return (None, dz if ctx.needs_input_grad[1] else None, None, None, None,
+                *_param_grads(mod, sv.store, gflat, live))
 
 
 # -------------------------------------------------------------------------------------------------

@@ -191,6 +191,19 @@ class FlatParamStore:
             return None
         return torch.as_strided(g, (self.total,), (1,), storage_offset=start)
 
+    def live_grad_buffer(self, params):
+        """The flat gradient buffer a backward should add into, or None: the buffer whose slices the .grads of EVERY one
+        of `params` (the trainable members of this store) already are - an earlier backward since zero_grad(), i.e. a
+        second probe call of one step or the next micro-batch of gradient accumulation.  Statistics cached for it are
+        dropped, since the caller is about to write it."""
+        params = list(params)
+        if not params or any(p.grad is None for p in params):
+            return None
+        gflat = self.grad_buffer(params)
+        if gflat is not None:
+            self.grads_changed()
+        return gflat
+
     def grad_sumsq(self, gflat, inv_scale=None, found_inf=None):
         """Per-tensor sums of squares of the gradient buffer `gflat`, one per trainable tensor (in segments()[1] order).
         With inv_scale (GradScaler's unscale) the same pass unscales gflat in place and raises found_inf on a non-finite

@@ -55,12 +55,10 @@ def _store_of(module, anchor):
 
 def _grad_buffer(store, members):
     """The flat gradient buffer of this step: the one the members' .grad already alias (an earlier probe call of the
-    same step), else a new zero buffer."""
-    if all(p.grad is not None for _, p in members):
-        gflat = store.grad_buffer(p for _, p in members)
-        if gflat is not None:
-            store.grads_changed()
-            return gflat
+    same step, or an earlier micro-batch under gradient accumulation), else a new zero buffer."""
+    gflat = store.live_grad_buffer(p for _, p in members)
+    if gflat is not None:
+        return gflat
     gflat = store.new_grad_buffer()
     for n, p in members:
         p.grad = store.grad_view(gflat, n)
