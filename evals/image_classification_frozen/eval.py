@@ -14,6 +14,7 @@ reference does and builds the classifier to follow it, exactly as in the video e
 
 `optimization.multihead_kwargs` trains several probes on one encoder pass per batch, with the video evaluation's parser,
 head construction, checkpoint and CSV layout (read_multihead_kwargs, build_heads, train_heads).
+`optimization.probe_depth` (default 1) sets every head's AttentiveClassifier depth, as in the video evaluation.
 """
 import os
 
@@ -34,7 +35,7 @@ import torch.nn.functional as F
 import src.models.vision_transformer as vit
 from evals.video_classification_frozen.eval import (  # noqa: F401  (the helpers both evaluations share)
     build_heads, init_opt, load_checkpoint, load_pretrained, loop_autocast, one_head, read_fp16_autocast,
-    read_multihead_kwargs, require_cuda, run_head_loop, step_head, train_heads)
+    read_multihead_kwargs, read_probe_depth, require_cuda, run_head_loop, step_head, train_heads)
 from src.datasets.data_manager import init_data
 from src.models.attentive_pooler import AttentiveClassifier
 from src.utils.distributed import init_distributed
@@ -86,6 +87,7 @@ def main(args_eval, resume_preempt=False):
     use_bfloat16 = args_opt.get('use_bfloat16')
     fp16_autocast = read_fp16_autocast(args_opt)
     multihead_kwargs = read_multihead_kwargs(args_opt)
+    probe_depth = read_probe_depth(args_opt)
 
     resume_checkpoint = args_eval.get('resume_checkpoint', False) or resume_preempt
     eval_tag = args_eval.get('tag', None)
@@ -118,7 +120,7 @@ def main(args_eval, resume_preempt=False):
 
     settings = multihead_kwargs or [one_head(wd, start_lr, lr, final_lr, warmup)]
     classifiers = build_heads(lambda: AttentiveClassifier(embed_dim=encoder.embed_dim, num_heads=encoder.num_heads,
-                                                          depth=1, num_classes=num_classes,
+                                                          depth=probe_depth, num_classes=num_classes,
                                                           follow_autocast=fp16_autocast).to(device), len(settings))
 
     train_loader = make_dataloader(dataset_name=dataset_name, root_path=root_path, resolution=resolution,

@@ -22,6 +22,9 @@ warmup, read by read_multihead_kwargs) trains several probes ("heads") on one en
 from the same weights and has its own optimizer, schedules, GradScaler and gradient exchange.  Without the key the
 driver trains one classifier with the reference's checkpoint, CSV and log lines.  Both cases, and the image evaluation,
 run the same epoch loop (train_heads) and batch loop (run_head_loop).
+
+`optimization.probe_depth` (default 1) builds every head as AttentiveClassifier(depth=probe_depth): depth - 1
+self-attention Blocks after the cross-attention block, whose parameters add `pooler.blocks.*` keys to the checkpoint.
 """
 import collections.abc
 import contextlib
@@ -114,6 +117,7 @@ def main(args_eval, resume_preempt=False):
     use_bfloat16 = args_opt.get('use_bfloat16')
     fp16_autocast = read_fp16_autocast(args_opt)
     multihead_kwargs = read_multihead_kwargs(args_opt)
+    probe_depth = read_probe_depth(args_opt)
 
     resume_checkpoint = args_eval.get('resume_checkpoint', False) or resume_preempt
     eval_tag = args_eval.get('tag', None)
@@ -157,7 +161,7 @@ def main(args_eval, resume_preempt=False):
 
     settings = multihead_kwargs or [one_head(wd, start_lr, lr, final_lr, warmup)]
     classifiers = build_heads(lambda: AttentiveClassifier(embed_dim=encoder.embed_dim, num_heads=encoder.num_heads,
-                                                          depth=1, num_classes=num_classes,
+                                                          depth=probe_depth, num_classes=num_classes,
                                                           follow_autocast=fp16_autocast).to(device), len(settings))
 
     train_loader = make_dataloader(dataset_type=dataset_type, root_path=train_data_path, resolution=resolution,
@@ -195,6 +199,15 @@ def read_fp16_autocast(args_opt):
     value = args_opt.get('fp16_autocast', False)
     if not isinstance(value, bool):
         raise ValueError(f"optimization.fp16_autocast must be true or false, got {value!r}")
+    return value
+
+
+def read_probe_depth(args_opt):
+    """`optimization.probe_depth` (default 1, the reference's eval.py:182-187): the depth of every head's
+    AttentiveClassifier, i.e. depth - 1 self-attention Blocks over the query token after the cross-attention block."""
+    value = args_opt.get('probe_depth', 1)
+    if isinstance(value, bool) or not isinstance(value, int) or value < 1:
+        raise ValueError(f"optimization.probe_depth must be an integer >= 1, got {value!r}")
     return value
 
 

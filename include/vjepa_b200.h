@@ -214,6 +214,21 @@ int vj_cross_attn_fwd_lse_f16(const void* q, const void* kv, void* out, float* l
 int vj_cross_attn_bwd_f16(const void* q, const void* kv, const void* out, const void* dout, const float* lse2, float* dq,
                           void* dkv, void* workspace, size_t ws_bytes, int B, int nq, int S, int H, int HD, float scale,
                           void* stream);
+/* Self-attention among each clip's nq query tokens: Attention.forward (src/models/utils/modules.py:61-78) of the
+ * depth - 1 Blocks of AttentivePooler(depth > 1) (src/models/attentive_pooler.py:52-102).  qkv bf16 [B*nq, 3*H*HD] is
+ * the Block's qkv Linear output (q | k | v thirds, head-major); out bf16 [B*nq, H*HD] = softmax(q k^T * scale) v per
+ * (clip, head).  lse2 fp32 [B*nq, H] (log2 domain, as vj_cross_attn_fwd_lse) may be null.  nq <= 128,
+ * HD in {32, 64, 80, 88, 104, 128}.  With nq = 1, out is bitwise v. */
+int vj_query_attn_fwd(const void* qkv, void* out, float* lse2, int B, int nq, int H, int HD, float scale, void* stream);
+/* Backward of the above from qkv, out, dout bf16 [B*nq, H*HD] and lse2: dqkv bf16 [B*nq, 3*H*HD] in qkv's layout.
+ * Deterministic: no atomics, every dqkv element is written once in a fixed summation order. */
+int vj_query_attn_bwd(const void* qkv, const void* out, const void* dout, const float* lse2, void* dqkv, int B, int nq,
+                      int H, int HD, float scale, void* stream);
+/* The two above with fp16 qkv / out / dout / dqkv (lse2 stays fp32): the Blocks under the evals' autocast(float16). */
+int vj_query_attn_fwd_f16(const void* qkv, void* out, float* lse2, int B, int nq, int H, int HD, float scale,
+                          void* stream);
+int vj_query_attn_bwd_f16(const void* qkv, const void* out, const void* dout, const float* lse2, void* dqkv, int B,
+                          int nq, int H, int HD, float scale, void* stream);
 
 /* ---- flat-buffer parameter kernels ------------------------------------------------------------ */
 /* dst bf16[n] = src fp32[n]: the per-step bf16 shadow of the fp32 master weights (what autocast's

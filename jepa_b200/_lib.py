@@ -55,6 +55,10 @@ SIGNATURES = {
     "vj_cross_attn_fwd_f16": (I, [P, P, P, I, I, I, I, I, F, P]),
     "vj_cross_attn_fwd_lse_f16": (I, [P, P, P, P, I, I, I, I, I, F, P]),
     "vj_cross_attn_bwd_f16": (I, [P, P, P, P, P, P, P, P, Z, I, I, I, I, I, F, P]),
+    "vj_query_attn_fwd": (I, [P, P, P, I, I, I, I, F, P]),
+    "vj_query_attn_fwd_f16": (I, [P, P, P, I, I, I, I, F, P]),
+    "vj_query_attn_bwd": (I, [P, P, P, P, P, I, I, I, I, F, P]),
+    "vj_query_attn_bwd_f16": (I, [P, P, P, P, P, I, I, I, I, F, P]),
     "vj_token_std_bwd": (I, [P, P, P, F, P, I, I, I, F, F, P]),
     "vj_cast_f32_bf16": (I, [P, P, L, P]),
     "vj_cast_f32_f16": (I, [P, P, L, P]),

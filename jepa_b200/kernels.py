@@ -309,6 +309,39 @@ def cross_attn_bwd(q, kv, out, dout, lse2, dq, dkv, B, nq, S, H, hd, scale):
     return dq, dkv
 
 
+QUERY_ATTN_MAX_TOKENS = 128
+
+
+def _query_attn_check(qkv, B, nq, H, hd):
+    if nq > QUERY_ATTN_MAX_TOKENS:
+        raise _lib.VJError(f"query_attn: nq = {nq} query tokens per clip; at most {QUERY_ATTN_MAX_TOKENS} are supported")
+    if qkv.dim() != 2 or qkv.shape[0] < B * nq or qkv.shape[1] != 3 * H * hd:
+        raise _lib.VJError(f"query_attn: qkv must be [>= {B * nq}, {3 * H * hd}], got {tuple(qkv.shape)}")
+
+
+def query_attn_fwd(qkv, out, lse2, B, nq, H, hd, scale):
+    """softmax(q k^T scale) v among each clip's nq tokens (the probe's Blocks, modules.py:61-78), q / k / v read from the
+    qkv Linear output [B*nq, 3*H*hd]; out [B*nq, H*hd] and qkv both bf16 or both fp16; lse2 fp32 [B*nq, H] or None."""
+    name = _f16("vj_query_attn_fwd", qkv)
+    _chk(qkv, None, "qkv"); _chk(out, qkv.dtype, "out")
+    if lse2 is not None:
+        _chk(lse2, F32, "lse2")
+    _query_attn_check(qkv, B, nq, H, hd)
+    _lib.call(name, _p(qkv), _p(out), _p(lse2), B, nq, H, hd, float(scale), _s())
+    return out
+
+
+def query_attn_bwd(qkv, out, dout, lse2, dqkv, B, nq, H, hd, scale):
+    """dqkv [B*nq, 3*H*hd] (qkv's layout and dtype) of query_attn_fwd."""
+    name = _f16("vj_query_attn_bwd", qkv)
+    for t, n in ((qkv, "qkv"), (out, "out"), (dout, "dout"), (dqkv, "dqkv")):
+        _chk(t, qkv.dtype, n)
+    _chk(lse2, F32, "lse2")
+    _query_attn_check(qkv, B, nq, H, hd)
+    _lib.call(name, _p(qkv), _p(out), _p(dout), _p(lse2), _p(dqkv), B, nq, H, hd, float(scale), _s())
+    return dqkv
+
+
 def token_std_accum(z, pstd, weight, eps=1e-4):
     _chk(z, BF16, "z"); _chk(pstd, F32, "pstd")
     B, K, D = z.shape

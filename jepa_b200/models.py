@@ -48,7 +48,7 @@ class Attention(nn.Module):
             raise NotImplementedError("dropout is not part of the accelerated path (all V-JEPA configs use 0)")
         if not qkv_bias:
             raise NotImplementedError("qkv_bias=False is not used by any V-JEPA factory")
-        if qk_scale is not None:
+        if qk_scale:      # None or False (AttentivePooler's Blocks) mean the default hd^-0.5, as `qk_scale or ...` does
             raise NotImplementedError("qk_scale override is not supported")
         self.num_heads = num_heads
         self.scale = (dim // num_heads) ** -0.5

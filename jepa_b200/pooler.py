@@ -11,9 +11,14 @@ Training the probe (the frozen evaluations' job, eval.py:317-373): with paramete
 what the backward needs and returns outputs with a grad_fn.  The probe's parameters live in one FlatParamStore (fp32
 master weights, bf16 GEMM operands in its shadow) and the backward writes ONE flat fp32 gradient buffer, so FlatAdamW,
 FlatGradScaler and step.clip_grad_norm_ each take one launch over it.  Several probe calls in one step (one per temporal
-segment without attend_across_segments) accumulate into the same buffer.  `proj` gets no gradient: the reference builds
-it but never applies it (modules.py:152-153).  Gradients into the encoder's tokens (fine-tuning) and depth > 1 are not
-implemented.
+segment without attend_across_segments) accumulate into the same buffer.  The cross-attention's `proj` gets no gradient:
+the reference builds it but never applies it (modules.py:152-153).  Gradients into the encoder's tokens (fine-tuning) are
+not implemented.
+
+depth = d adds d - 1 transformer Blocks (modules.py:81-120) after the cross-attention block, self-attention over the
+num_queries query tokens of each clip (attentive_pooler.py:52-60, 100-101): LayerNorm, GEMMs with the same epilogues, and
+`vj_query_attn_fwd` / `vj_query_attn_bwd` for the attention (num_queries <= 128).  Their residual stream stays fp32, and
+their parameters live in the same FlatParamStore and flat gradient buffer as the rest of the probe.
 
 Precision: the probe computes bf16 x bf16 -> fp32 by default, inside an autocast region or not.  Built with
 `follow_autocast=True`, it follows an fp16 autocast (torch.autocast('cuda', dtype=torch.float16) or
@@ -31,7 +36,7 @@ import torch
 import torch.nn as nn
 
 from . import kernels as K
-from .models import MLP, VisionTransformer
+from .models import MLP, Block, VisionTransformer
 from .params import FlatParamStore
 from .pos_embs import get_1d_sincos_pos_embed
 from .tensors import apply_masks, trunc_normal_
@@ -97,9 +102,12 @@ class AttentivePooler(nn.Module):
                  init_std=0.02, qkv_bias=True, complete_block=True, follow_autocast=False):
         super().__init__()
         self.follow_autocast = follow_autocast       # a plain attribute: not a parameter, not in the state_dict
-        if depth != 1:
-            raise NotImplementedError("AttentivePooler depth > 1 (extra self-attention blocks over the query tokens) is not "
-                                      "used by the frozen evaluations (eval.py:182-187 builds depth=1)")
+        if depth > 1 and not qkv_bias:
+            raise NotImplementedError("AttentivePooler depth > 1 with qkv_bias=False: the probe's self-attention Blocks "
+                                      "run with qkv biases only")
+        if depth > 1 and num_queries > K.QUERY_ATTN_MAX_TOKENS:
+            raise NotImplementedError(f"AttentivePooler depth > 1 with num_queries = {num_queries}: vj_query_attn_fwd "
+                                      f"supports at most {K.QUERY_ATTN_MAX_TOKENS} query tokens")
         if embed_dim % num_heads or (embed_dim // num_heads) not in (32, 64, 80, 88, 104, 128):
             raise NotImplementedError(f"head dim {embed_dim // num_heads}: vj_cross_attn_fwd supports 32 / 64 / 80 / 88 / "
                                       "104 / 128")
@@ -111,6 +119,9 @@ class AttentivePooler(nn.Module):
         else:
             self.cross_attention_block = CrossAttention(dim=embed_dim, num_heads=num_heads, qkv_bias=qkv_bias)
         self.blocks = None
+        if depth > 1:
+            self.blocks = nn.ModuleList([Block(dim=embed_dim, num_heads=num_heads, mlp_ratio=mlp_ratio, qkv_bias=qkv_bias,
+                                               qk_scale=False, norm_layer=norm_layer) for _ in range(depth - 1)])
         self.init_std = init_std
         self.embed_dim, self.num_heads, self.num_queries = embed_dim, num_heads, num_queries
         trunc_normal_(self.query_tokens, std=self.init_std)
@@ -127,6 +138,10 @@ class AttentivePooler(nn.Module):
             rescale(self.cross_attention_block.mlp.fc2.weight.data, 1)
         else:
             rescale(self.cross_attention_block.proj.weight.data, 1)
+        if self.blocks is not None:
+            for layer_id, layer in enumerate(self.blocks, 1):
+                rescale(layer.attn.proj.weight.data, layer_id + 1)
+                rescale(layer.mlp.fc2.weight.data, layer_id + 1)
 
     def _init_weights(self, m):
         if isinstance(m, nn.Linear):
@@ -189,7 +204,7 @@ class _ProbeFn(torch.autograd.Function):
     """forward: the probe on the kernels, saving its activations.  backward: accumulates every trainable parameter's
     gradient into the store's flat gradient buffer of this step (and points .grad at its slices) - a flat buffer that two
     probe calls of one step can share, which autograd's per-tensor accumulation would break apart - and returns None for
-    the parameters.  proj is left without a gradient, as in the reference."""
+    the parameters.  The cross-attention's proj is left without a gradient, as in the reference."""
 
     @staticmethod
     def forward(ctx, pooler, store, prefix, x, head, dt, sync, *params):
@@ -201,7 +216,7 @@ class _ProbeFn(torch.autograd.Function):
     @staticmethod
     def backward(ctx, dy):
         pooler, store, prefix, sv = ctx.pooler, ctx.store, ctx.prefix, ctx.sv
-        members = [(p._vj_name, p) for p in ctx.params if p.requires_grad and ".proj." not in p._vj_name]
+        members = [(p._vj_name, p) for p in ctx.params if p.requires_grad and not _unapplied(p._vj_name)]
         if members:
             gflat = _grad_buffer(store, members)
             _probe_backward(pooler, store, prefix, sv, dy, ctx.head, gflat)
@@ -210,6 +225,11 @@ class _ProbeFn(torch.autograd.Function):
         n = len(ctx.params)
         ctx.sv = ctx.params = ctx.sync = None
         return (None,) * 7 + (None,) * n
+
+
+def _unapplied(name):
+    """The cross-attention's proj: built and checkpointed, never applied (modules.py:152-153)."""
+    return ".proj." in name and "cross_attention_block." in name
 
 
 def _names(pooler, prefix):
@@ -265,6 +285,7 @@ def _probe_forward(pooler, store, prefix, x, head, save, dt=BF16):
     M = _pad_rows(B * nq, 8)
     if not pooler.complete_block:
         pooled = att.clone() if dt == F16 else att.float()     # SDPA's output dtype under fp16 autocast (att is saved)
+        q2 = None
     else:
         # q = q + y ; q = q + fc2(gelu(fc1(norm2(q))))   (fp32 residual stream: it is only B*nq rows)
         q1p = torch.zeros(M, D, dtype=F32, device=dev)
@@ -285,6 +306,16 @@ def _probe_forward(pooler, store, prefix, x, head, save, dt=BF16):
         pooled = q2[:B * nq]
         if save:
             sv.q1p, sv.ln2, sv.mean2, sv.rstd2, sv.h, sv.g = q1p, ln2, mean2, rstd2, h, g
+    if pooler.blocks is not None:
+        if q2 is None:
+            q2 = torch.zeros(M, D, dtype=F32, device=dev)
+            q2[:B * nq] = att.float()
+        q2, blocks_sv = _blocks_forward(pooler, store, prefix, q2, B, save, dt)
+        pooled = q2[:B * nq]
+        if not pooler.complete_block and dt == F16:       # the reference's residual stream is fp16 there
+            pooled = pooled.to(F16)
+        if save:
+            sv.blocks = blocks_sv
     if not head:
         return pooled.view(B, nq, D), sv
     # linear head as logits^T [C, Np] = W [C, D] . pooled^T: the GEMM's N is the (padded) batch, so the weight is read
@@ -333,6 +364,8 @@ def _probe_backward(pooler, store, prefix, sv, dy, head, gflat):
     else:
         dq2 = torch.zeros(Mp, D, dtype=F32, device=dev)
         dq2[:M] = dy.detach().reshape(M, D)
+    if pooler.blocks is not None:
+        dq2 = _blocks_backward(pooler, store, prefix, sv.blocks, dq2, B, gflat, dt)
     if pooler.complete_block:
         # MLP: q2 = q1 + fc2(gelu(fc1(ln2(q1))))
         dq2b = dq2.to(dt)
@@ -375,6 +408,83 @@ def _probe_backward(pooler, store, prefix, sv, dy, head, gflat):
         dx = torch.empty_like(sv.x2)
         K.layernorm_bwd(dxn, sv.x2, f(blk + "norm1.weight"), sv.mean1, sv.rstd1, None, dx, gv(blk + "norm1.weight"),
                         gv(blk + "norm1.bias"))
+
+
+def _blocks_forward(pooler, store, prefix, x, B, save, dt):
+    """The depth - 1 Blocks over the query tokens (attentive_pooler.py:100-101, Block.forward of modules.py:114-120) on
+    the fp32 residual stream x [M, D] (B*nq rows, padded to 8): x = x + proj(attn(norm1(x))); x = x + mlp(norm2(x)).
+    Returns (x after the last Block, per-Block saved activations or None)."""
+    M, D = x.shape
+    H, nq, dev = pooler.num_heads, pooler.num_queries, x.device
+    w = lambda name: store.w16(name, dt)
+    f = store.f32
+    saved = [] if save else None
+    for i, blk in enumerate(pooler.blocks):
+        n = f"{prefix}blocks.{i}."
+        xn = torch.empty(M, D, dtype=dt, device=dev)
+        mean1 = torch.empty(M, dtype=F32, device=dev) if save else None
+        rstd1 = torch.empty(M, dtype=F32, device=dev) if save else None
+        K.layernorm_fwd(x, xn, f(n + "norm1.weight"), f(n + "norm1.bias"), blk.norm1.eps, mean1, rstd1)
+        qkv = torch.empty(M, 3 * D, dtype=dt, device=dev)
+        K.gemm(xn, w(n + "attn.qkv.weight"), qkv, bias=f(n + "attn.qkv.bias"))
+        att = torch.zeros(M, D, dtype=dt, device=dev)          # the pad rows feed the proj GEMM: zeros
+        lse2 = torch.empty(B * nq, H, dtype=F32, device=dev) if save else None
+        K.query_attn_fwd(qkv, att, lse2, B, nq, H, D // H, blk.attn.scale)
+        x1 = torch.empty(M, D, dtype=F32, device=dev)
+        K.gemm(att, w(n + "attn.proj.weight"), x1, bias=f(n + "attn.proj.bias"), epi=K.EPI_ADD, aux=x)
+        ln2 = torch.empty(M, D, dtype=dt, device=dev)
+        mean2 = torch.empty(M, dtype=F32, device=dev) if save else None
+        rstd2 = torch.empty(M, dtype=F32, device=dev) if save else None
+        K.layernorm_fwd(x1, ln2, f(n + "norm2.weight"), f(n + "norm2.bias"), blk.norm2.eps, mean2, rstd2)
+        hid = store.offsets[n + "mlp.fc1.weight"][2][0]
+        g = torch.empty(M, hid, dtype=dt, device=dev)
+        h = torch.empty(M, hid, dtype=dt, device=dev) if save else None
+        K.gemm(ln2, w(n + "mlp.fc1.weight"), g, bias=f(n + "mlp.fc1.bias"), epi=K.EPI_GELU_GRAD if save else K.EPI_GELU,
+               aux_out=h)
+        x2 = torch.empty(M, D, dtype=F32, device=dev)
+        K.gemm(g, w(n + "mlp.fc2.weight"), x2, bias=f(n + "mlp.fc2.bias"), epi=K.EPI_ADD, aux=x1)
+        if save:
+            saved.append(SimpleNamespace(x=x, xn=xn, mean1=mean1, rstd1=rstd1, qkv=qkv, att=att, lse2=lse2, x1=x1,
+                                         ln2=ln2, mean2=mean2, rstd2=rstd2, h=h, g=g))
+        x = x2
+    return x, saved
+
+
+def _blocks_backward(pooler, store, prefix, saved, dx, B, gflat, dt):
+    """Backward of _blocks_forward: adds every Block parameter's gradient into gflat and returns the fp32 gradient
+    [M, D] into the first Block's input."""
+    M, D = dx.shape
+    H, nq, dev = pooler.num_heads, pooler.num_queries, dx.device
+    w = lambda name: store.w16(name, dt)
+    f = store.f32
+    gv = lambda name: store.grad_view(gflat, name)
+    for i in reversed(range(len(pooler.blocks))):
+        n, s = f"{prefix}blocks.{i}.", saved[i]
+        # MLP: x2 = x1 + fc2(gelu(fc1(norm2(x1))))
+        dxb = dx.to(dt)
+        _wgrad(dxb, s.g, gv(n + "mlp.fc2.weight"), gv(n + "mlp.fc2.bias"), M)
+        dpre = torch.empty(M, s.g.shape[1], dtype=dt, device=dev)
+        K.gemm(dxb, w(n + "mlp.fc2.weight"), dpre, b_mn=True, epi=K.EPI_MUL, aux=s.h)
+        _wgrad(dpre, s.ln2, gv(n + "mlp.fc1.weight"), gv(n + "mlp.fc1.bias"), M)
+        dln2 = torch.empty(M, D, dtype=dt, device=dev)
+        K.gemm(dpre, w(n + "mlp.fc1.weight"), dln2, b_mn=True)
+        dx1 = torch.empty(M, D, dtype=F32, device=dev)
+        K.layernorm_bwd(dln2, s.x1, f(n + "norm2.weight"), s.mean2, s.rstd2, dx, dx1, gv(n + "norm2.weight"),
+                        gv(n + "norm2.bias"))
+        # attention: x1 = x + proj(attn(qkv(norm1(x))))
+        dx1b = dx1.to(dt)
+        _wgrad(dx1b, s.att, gv(n + "attn.proj.weight"), gv(n + "attn.proj.bias"), M)
+        datt = torch.empty(M, D, dtype=dt, device=dev)
+        K.gemm(dx1b, w(n + "attn.proj.weight"), datt, b_mn=True)
+        dqkv = torch.zeros(M, 3 * D, dtype=dt, device=dev)     # the pad rows feed the qkv wgrad: zeros
+        K.query_attn_bwd(s.qkv, s.att, datt, s.lse2, dqkv, B, nq, H, D // H, pooler.blocks[i].attn.scale)
+        _wgrad(dqkv, s.xn, gv(n + "attn.qkv.weight"), gv(n + "attn.qkv.bias"), M)
+        dxn = torch.empty(M, D, dtype=dt, device=dev)
+        K.gemm(dqkv, w(n + "attn.qkv.weight"), dxn, b_mn=True)
+        dx = torch.empty(M, D, dtype=F32, device=dev)
+        K.layernorm_bwd(dxn, s.x, f(n + "norm1.weight"), s.mean1, s.rstd1, dx1, dx, gv(n + "norm1.weight"),
+                        gv(n + "norm1.bias"))
+    return dx
 
 
 def _wgrad(dy, act, grad_out, bias_grad, tokens):

@@ -2,7 +2,7 @@
 """Frozen-evaluation probe training step (or validation step), clips/sec, at the ViT-L/16 K400 shape.
 
     python tools/bench_probe.py [--steps K] [--warmup W] [--batch B] [--mode train|val|image|xattn]
-                                [--dtype bfloat16|float16] [--heads 1,4,16]
+                                [--dtype bfloat16|float16] [--heads 1,4,16] [--depth 1,2,4]
 
 --heads (train, val, image) runs the evaluation loop with several probes on one encoder pass
 (optimization.multihead_kwargs): per step the encoder runs once, then every probe its forward (+ backward, GradScaler,
@@ -13,6 +13,12 @@ those of the first count.
 --dtype float16 runs each step's encoder and classifier calls inside the reference's autocast(dtype=torch.float16)
 region (evals/video_classification_frozen/eval.py:323) with AttentiveClassifier(follow_autocast=True): fp16 encoder,
 fp16 probe forward and backward, fp16 logits, GradScaler.  The default bfloat16 is the evaluation loop without autocast.
+
+--depth 1,2,4 times the probe alone (AttentiveClassifier(depth=d), ViT-L width, K400 classes) on device-resident
+encoder tokens [B, 12544, 1024]: forward + backward + GradScaler unscale, clip and FlatAdamW step per training step, the
+listed depths alternating step by step.  It also times vj_query_attn_fwd / _bwd alone (CUDA events around a CUDA graph of
+200 back-to-back launches) at that shape's one query token per clip, and at 16 query tokens (an AttentivePooler with
+num_queries=16).
 
 --mode xattn times vj_cross_attn_fwd_lse and vj_cross_attn_bwd alone, bf16 and fp16 alternating, at the K400 probe
 shapes (B 4, S 12 544, one query; ViT-L H 16 x hd 64 and ViT-H H 16 x hd 80), and reports GB/s from the bytes each must
@@ -244,6 +250,81 @@ def _reference_cpu_ms(clip, crop):
         return round(float(r.stdout.strip().splitlines()[-1]), 1)
     except (ValueError, IndexError):
         return None
+
+
+def run_depth(args):
+    from jepa_b200 import kernels as Kn
+    from jepa_b200.optim import FlatAdamW, FlatGradScaler
+    from jepa_b200.pooler import AttentiveClassifier
+    from jepa_b200.step import clip_grad_norm_
+    device = torch.device("cuda:0")
+    torch.manual_seed(0)
+    B, S, D, H, n_cls = args.batch, 12544, 1024, 16, 400
+    fp16 = args.dtype == "float16"
+    probes = {}
+    for d in args.depth:
+        clf = AttentiveClassifier(embed_dim=D, num_heads=H, depth=d, num_classes=n_cls, follow_autocast=fp16).to(device)
+        groups = [{"params": [p for n, p in clf.named_parameters() if ("bias" not in n) and (len(p.shape) != 1)]},
+                  {"params": [p for n, p in clf.named_parameters() if ("bias" in n) or (len(p.shape) == 1)],
+                   "WD_exclude": True, "weight_decay": 0}]
+        probes[d] = (clf, FlatAdamW(groups, lr=1e-3, weight_decay=0.01), FlatGradScaler())
+    crit = torch.nn.CrossEntropyLoss()
+    tokens = torch.randn(B, S, D, device=device)
+    labels = torch.randint(0, n_cls, (B,), device=device)
+    ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    times = {d: [] for d in args.depth}
+    for i in range(args.warmup + args.steps):
+        for d in args.depth:            # alternate the depths step by step: clock drift spreads over all of them
+            clf, opt, scaler = probes[d]
+            ev0.record()
+            with _region(args):
+                loss = crit(clf(tokens), labels)
+            scaler.scale(loss).backward()
+            scaler.unscale_(opt)
+            clip_grad_norm_(clf, 1.0)
+            scaler.step(opt)
+            scaler.update()
+            opt.zero_grad()
+            ev1.record()
+            torch.cuda.synchronize()
+            if i >= args.warmup:
+                times[d].append(ev0.elapsed_time(ev1))
+    med = lambda xs: sorted(xs)[len(xs) // 2]
+    dt = torch.float16 if fp16 else torch.bfloat16
+    kern = []
+    for nq in (1, 16):
+        qkv = torch.randn(B * nq, 3 * D, device=device).to(dt)
+        out = torch.empty(B * nq, D, dtype=dt, device=device)
+        dout = torch.randn(B * nq, D, device=device).to(dt)
+        lse = torch.empty(B * nq, H, device=device)
+        dqkv = torch.empty_like(qkv)
+        row = {"nq": nq}
+        for name, fn in (("fwd_us", lambda: Kn.query_attn_fwd(qkv, out, lse, B, nq, H, D // H, (D // H) ** -0.5)),
+                         ("bwd_us", lambda: Kn.query_attn_bwd(qkv, out, dout, lse, dqkv, B, nq, H, D // H,
+                                                              (D // H) ** -0.5))):
+            for _ in range(20):
+                fn()
+            torch.cuda.synchronize()
+            # replayed from a CUDA graph: the launches run back to back on the device, so the events time the kernels
+            # rather than the host's ctypes dispatch of each call
+            reps, replays = 200, 5
+            graph = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(graph):
+                for _ in range(reps):
+                    fn()
+            graph.replay()
+            ev0.record()
+            for _ in range(replays):
+                graph.replay()
+            ev1.record()
+            torch.cuda.synchronize()
+            row[name] = round(ev0.elapsed_time(ev1) * 1000 / (reps * replays), 2)
+        kern.append(row)
+    card = _card()
+    print(json.dumps({"mode": "depth", "dtype": args.dtype, "batch": B, "tokens_per_clip": S, "width": D, "heads": H,
+                      "probe_step_ms": {str(d): round(med(t), 3) for d, t in times.items()},
+                      "query_attn_kernel": kern, "steps": args.steps, "warmup": args.warmup,
+                      "gpu": card[0] if card else None, "power_limit_w": card[1] if len(card) > 1 else None}))
 
 
 def _card():
@@ -578,6 +659,9 @@ def main():
                     help="train / val / image mode: comma-separated probe counts trained (validated) on one encoder "
                          "pass, e.g. 1,4,16, alternated step by step; reports encoder ms, probe ms per head and "
                          "throughput for each")
+    ap.add_argument("--depth", default=None,
+                    help="comma-separated probe depths, e.g. 1,2,4: ms per probe training step on device-resident "
+                         "tokens for each, and the query self-attention kernels alone")
     ap.add_argument("--head-dims", default="64,80",
                     help="xattn mode: comma-separated head dims timed, e.g. 80,88,104,128")
     args = ap.parse_args()
@@ -588,6 +672,13 @@ def main():
         ap.error("--heads: distinct positive head counts")
     if args.multi and args.mode == "xattn":
         ap.error("--heads applies to --mode train, val and image")
+    if args.depth is not None:
+        args.depth = [int(d) for d in args.depth.split(",")]
+        if any(d < 1 for d in args.depth) or len(set(args.depth)) != len(args.depth):
+            ap.error("--depth: distinct positive depths")
+        args.batch = args.batch or 4
+        run_depth(args)
+        return
     if args.mode == "image":
         run_image(args)
         return
